@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the hot path: batched witness generation (+ R1CS check) on B200.
+"""Benchmark of the hot path: batched witness generation (+ R1CS check) on an H100.
 
   python bench.py --gpus N --steps K --warmup W          our arm (one process per GPU under torchrun)
   python bench.py --impl reference ...                   the reference's CPU path on the host cores
+  python bench.py --dump-outputs DIR ...                 also write what the last timed step computed (.npy)
 
 Metric (BASELINE.json): witnesses/s on the ~1M-constraint BN254 circuit; the R1CS check is reported
 beside it as Mconstraints/s.  A step = one pass of the hot path over one batch of synthetic inputs:
@@ -18,6 +19,10 @@ Besides the headline workload the JSON line carries `configs`: every BASELINE.js
 per-GPU batch (C2 Sha256compression x1024, C3 ecdsa-scale x8, C4 Sha256(512)/BLS12-381 x1024 + R1CS), each with
 value / e2e / roofline and a `parity` field that is "ok" only after sampled witnesses of THAT run were compared
 byte for byte with the reference calculator's .wtns for the same inputs.
+
+The default batch of the headline workload is one full wave of warp-per-op tiles on the device it runs on
+(SMs x 4 CTAs x 32 instances: 16,896 on an H100 SXM).  Inputs are seeded, so runs with the same arguments on
+the same GPU model compute the same witnesses; `--dump-outputs` makes that comparable between two builds.
 """
 from __future__ import annotations
 
@@ -32,6 +37,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
+
+sys.dont_write_bytecode = True   # the tree may be read-only; nothing is written into it
 
 WORKLOADS = ["ecdsa_scale", "sha256compression", "poseidon2", "sha256_512_bls", "ecdsa_scale_calls"]
 
@@ -55,7 +62,30 @@ def parse_args():
     ap.add_argument("--no-gather", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-seconds", type=float, default=20.0)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step of the headline workload as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
+
+
+def sm_count() -> int:
+    """streaming multiprocessors of the current GPU (the C library sizes its tiles and grids by the same count)"""
+    import torch
+    if not torch.cuda.is_available():
+        return 132   # H100 SXM: only the size figures of the CPU-only reference arm use it
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+def wave_batch() -> int:
+    """one full wave of warp-per-op tiles: SMs x 4 CTAs x 32 instances (2.2 MB of value store each)"""
+    return sm_count() * 4 * 32
+
+
+def warp_per_op_batch() -> int:
+    """the batch from which the C library runs 32 instances per tile (>= 2 tiles per SM, cw_batch_create)"""
+    return sm_count() * 2 * 32
 
 
 # ---------------------------------------------------------------------------------------------
@@ -70,14 +100,13 @@ def make_workload(args):
     if args.workload == "ecdsa_scale":
         d.set_main(C.ecdsa_scale(d, args.lanes, args.chain), "ecdsa_scale_%dx%d" % (args.lanes, args.chain))
         label = "ecdsa-scale synthetic (secp256k1 BigMultModP chains %dx%d, 4x64-bit limbs), BN254" % (args.lanes, args.chain)
-        # 18,944 = 148 SMs x 4 CTAs x 32 instances: one full wave of warp-per-op tiles; 2.2 MB of value store each
-        batch = args.batch_per_gpu or 18944
+        batch = args.batch_per_gpu or wave_batch()
     elif args.workload == "ecdsa_scale_calls":
         d.set_main(C.ecdsa_scale(d, args.lanes, args.chain, hints="functions"),
                    "ecdsa_scale_calls_%dx%d" % (args.lanes, args.chain))
         label = ("ecdsa-scale synthetic with function-computed hints (one long_div-style call per BigMultModP returns "
                  "quotient and remainder as `var out[9]`), %dx%d, BN254" % (args.lanes, args.chain))
-        batch = args.batch_per_gpu or 18944
+        batch = args.batch_per_gpu or wave_batch()
     elif args.workload == "sha256compression":
         d.set_main(C.sha256_compression(d), "sha256compression")
         label = "Sha256compression, BN254"
@@ -105,7 +134,7 @@ def synth_inputs(desc, workload: str, batch: int, seed: int) -> np.ndarray:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -158,19 +187,6 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def ncu_traffic(workload_name: str, batch: int, kernel: str):
-    """DRAM bytes per launch of `kernel` from the committed ncu capture, if it was taken on this configuration"""
-    for name in ("r02_traffic.json",):
-        try:
-            j = json.load(open(os.path.join(ROOT, "profiles", name)))
-            for rec in j["captures"]:
-                if rec["workload"] == workload_name and rec["batch_per_gpu"] == batch and kernel in rec:
-                    return int(rec[kernel]["dram_bytes_read"] + rec[kernel]["dram_bytes_write"])
-        except Exception:
-            pass
-    return None
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -179,7 +195,7 @@ def measured_peaks():
             return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 # ---------------------------------------------------------------------------------------------
@@ -302,6 +318,31 @@ def cpu_reference_run(desc, args, inputs: np.ndarray, seconds: float):
                       % (n, cores, dt, t1)}
 
 
+DUMP_INSTANCES = 8        # instances whose witness is written (0, the last one and a seeded sample)
+DUMP_ENTRIES = 65536      # witness entries per instance (a seeded sample when the witness is longer)
+
+
+def dump_outputs(out_dir: str, b, circuit, batch: int, status: np.ndarray) -> None:
+    """What a caller of the timed path receives, after its last step: the per-instance status and the witness rows
+    (canonical field elements).  A field element is written as its eight 32-bit limbs, little-endian, each an exact
+    float64; a fixed, seeded sample of instances and entries keeps the files below 64 MB."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(2024)
+    W = circuit.n_witness
+    inst = sorted({0, batch - 1} | {int(x) for x in rng.choice(batch, min(batch, DUMP_INSTANCES - 2), replace=False)})
+    inst = np.asarray(inst[:DUMP_INSTANCES], dtype=np.int64)
+    ent = np.sort(rng.choice(W, DUMP_ENTRIES, replace=False)) if W > DUMP_ENTRIES else np.arange(W)
+    rows = []
+    for i in inst:
+        raw = b.wtns_bytes(int(i))
+        rows.append(np.frombuffer(raw[len(raw) - 32 * W:], dtype=np.uint64).reshape(W, 4)[ent])
+    limbs = np.ascontiguousarray(np.stack(rows)).view(np.uint32).reshape(len(inst), len(ent), 8)
+    np.save(os.path.join(out_dir, "witness.npy"), limbs.astype(np.float64))
+    np.save(os.path.join(out_dir, "witness_instances.npy"), inst.astype(np.float64))
+    np.save(os.path.join(out_dir, "witness_entries.npy"), ent.astype(np.float64))
+    np.save(os.path.join(out_dir, "status.npy"), status.astype(np.float64))
+
+
 def native_lib():
     from circom_b200 import native
     return native.lib
@@ -341,7 +382,7 @@ class Ctx:
 
 def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e2e_steps: int, r1cs: bool,
                  parity_samples: int, lanes: int = 8, chain: int = 132, e2e_batch: int = 0, e2e_chunk: int = 0,
-                 sample_clocks: bool = False, gather: bool = False):
+                 sample_clocks: bool = False, gather: bool = False, dump_dir: str = ""):
     """one workload on every rank; returns the result dict on every rank (only rank 0's is printed)"""
     import torch
     import torch.distributed as dist
@@ -352,7 +393,7 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
     rank, world, dev = ctx.rank, ctx.world, ctx.local_rank
     # one-time collective: rank 0's circuit description is broadcast over NCCL (every rank lowers it: 0.2-2.4 s)
     blob = broadcast_blob(desc.to_bytes() if rank == 0 else None, rank, world, device="cuda")
-    fuse = batch >= 9472 if ctx.args.fuse < 0 else bool(ctx.args.fuse)   # measured: pays for warp-per-op batches only
+    fuse = batch >= warp_per_op_batch() if ctx.args.fuse < 0 else bool(ctx.args.fuse)   # pays for warp-per-op batches only
     circuit = Circuit(blob, fuse=fuse)
     st = circuit.stats
     b = Batch(circuit, batch, dev)
@@ -388,6 +429,8 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
     status = b.status()
     assert os.environ.get("CW_BENCH_NOCHECK") or not status.any(), "witness generation reported failing asserts: %r" % status[:8]
     bt_log2, threads, bytes_per_inst = b.layout()
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, b, circuit, batch, status)
 
     # ---- parity: sampled witnesses of this run against the reference calculator -------------------
     parity = None
@@ -402,7 +445,7 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
         r = R1cs(circuit)
         fb, _ = r.check_batch(b)
         assert (fb == -1).all(), "R1CS check failed on generated witnesses"
-        ms = [r.check_batch(b)[1] for _ in range(max(2, steps))]
+        ms = [r.check_batch(b)[1] for _ in range(steps)]
         r1cs_ms = ctx.max_over_ranks([float(np.mean(ms))])[0]
         try:   # which kernel decides the rows (integer rows: csrc/r1cs_small.h)
             r1cs_rows = r.compiled_info(b)
@@ -426,7 +469,7 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
         else:
             del b
             torch.cuda.empty_cache()
-            ecirc = Circuit(blob, fuse=False) if fuse and chunk < 9472 else circuit   # small chunks: one operator per work item
+            ecirc = Circuit(blob, fuse=False) if fuse and chunk < warp_per_op_batch() else circuit   # small chunks: one operator per work item
             pair = [Batch(ecirc, chunk, dev), Batch(ecirc, chunk, dev)]
         from circom_b200.witness_calculator import aligned_empty
         outs = [aligned_empty((chunk, W, 4)) for _ in range(2)]   # pageable, 64-byte aligned: first touched by the workers
@@ -501,7 +544,7 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
         "e2e": e2e,
         "gpu_launches": 2 * steps,   # stage_inputs_kernel + tape_exec_kernel per step
         "roofline": {"kernel": "tape_exec_kernel", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": ncu_traffic(desc.name, batch, "tape_exec_kernel"),
+                     "frac": achieved / peak,
                      "peak_source": peak_src, "algorithmic_bytes_per_witness": b_wit,
                      "basis": "SURVEY 8(d): 32 B per value written (comparable with round 1); the compact store moves less",
                      "layout_bytes_per_witness": layout_bytes,
@@ -524,7 +567,6 @@ def run_workload(ctx: Ctx, workload: str, batch: int, steps: int, warmup: int, e
                        "roofline": {"kernel": r1cs_kernel, "bound": "hbm",
                                     "achieved": b_r1cs / (r1cs_ms / 1e3) / 1e9, "peak": peak, "unit": "GB/s",
                                     "frac": b_r1cs / (r1cs_ms / 1e3) / 1e9 / peak,
-                                    "traffic": ncu_traffic(desc.name, batch, r1cs_kernel),
                                     "basis": "SURVEY 8(d): 32 B per wire and instance; the check reads the compact store "
                                              "(bits as bits, recomposition runs as words), so it moves far fewer bytes "
                                              "than that and is bound by integer issue",
@@ -569,15 +611,16 @@ def main():
     _, _, batch = make_workload(args)
     out, desc, inputs = run_workload(ctx, args.workload, batch, args.steps, args.warmup, e2e_steps, not args.no_r1cs,
                                      parity_samples=2, lanes=args.lanes, chain=args.chain, e2e_batch=args.e2e_batch,
-                                     e2e_chunk=args.e2e_chunk, sample_clocks=True, gather=not args.no_gather)
+                                     e2e_chunk=args.e2e_chunk, sample_clocks=True, gather=not args.no_gather,
+                                     dump_dir=args.dump_outputs)
     if not args.no_configs and args.workload == "ecdsa_scale":
         # every BASELINE.json config at its stated per-GPU batch, each parity-gated against the reference calculator
         cfgs = []
         plan = [("C2", "sha256compression", 1024, True, 4), ("C3", "ecdsa_scale", 8, True, 2),
                 ("C4", "sha256_512_bls", 1024, True, 4),
-                ("C3-calls: the headline circuit with its hints computed by circom-style functions", "ecdsa_scale_calls", 18944, False, 2)]
+                ("C3-calls: the headline circuit with its hints computed by circom-style functions", "ecdsa_scale_calls", batch, False, 2)]
         for tag, wl, bsz, r1, ps in plan:
-            res, d2, in2 = run_workload(ctx, wl, bsz, max(3, min(args.steps, 5)), 3, 1, r1, parity_samples=ps,
+            res, d2, in2 = run_workload(ctx, wl, bsz, args.steps, args.warmup, 1, r1, parity_samples=ps,
                                         lanes=args.lanes, chain=args.chain)
             res["config_id"] = tag
             if rank == 0 and world == 1 and not args.no_cpu_baseline and wl != args.workload:

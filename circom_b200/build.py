@@ -1,4 +1,4 @@
-"""Build libcircom_b200.so (CUDA kernels for sm_100a + C ABI) in-tree with nvcc."""
+"""Build libcircom_b200.so (CUDA kernels for sm_90a + C ABI) in-tree with nvcc."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,7 @@ CLI = os.path.join(HERE, "circom_cuda_witness")
 SOURCES = ["capi.cu", "tape_calls.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
 CLI_SOURCES = ["cli.cpp"]
 HEADERS = ["kernels.cuh", "fr_device.cuh", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 

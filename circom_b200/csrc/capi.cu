@@ -1,5 +1,5 @@
 // C ABI (include/circom_b200.h) over the lowering (flatten.cpp), the formats (formats.cpp) and the
-// sm_100a kernels (kernels.cuh).  There is no CPU execution path: every compute entry point
+// sm_90a kernels (kernels.cuh).  There is no CPU execution path: every compute entry point
 // returns CW_ENODEV when no CUDA device is present.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -87,6 +87,18 @@ int ensure_device(int device) {
         g_dev_ready[device] = true;
     }
     return CW_OK;
+}
+
+// streaming multiprocessors of the current device: the grid caps of the grid-stride kernels and the tile size
+// cw_batch_create picks are counted in SMs
+u32 device_sms() {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        n <= 0) {
+        cudaGetLastError();
+        return 132;   // H100 SXM
+    }
+    return (u32)n;
 }
 
 struct DevTape {
@@ -519,11 +531,12 @@ int cw_batch_create(const cw_circuit *c, uint32_t batch, int device, cw_batch **
     // along the ops of a level (one-instance tiles).
     int bt = env_int("CW_BT_LOG2", -1);
     const uint64_t avg_w = t.n_levels() ? t.n_items() / t.n_levels() + 1 : 1;
+    const u32 sms = device_sms();
     if (bt < 0) {
         bt = 0;
-        if (batch >= 32u * 148u * 2u) bt = 5;   // (also with function calls: the 32 lanes run the same function body)
+        if (batch >= 32u * sms * 2u) bt = 5;   // (also with function calls: the 32 lanes run the same function body)
         else if (t.call_tab.empty())
-            while (bt < 5 && (avg_w << bt) < 64 && (batch >> (bt + 1)) >= 296u) ++bt;  // very narrow tapes (Poseidon)
+            while (bt < 5 && (avg_w << bt) < 64 && (batch >> (bt + 1)) >= 2u * sms) ++bt;  // very narrow tapes (Poseidon)
     }
     if (bt > 5) bt = 5;
     b->bt_log2 = (u32)bt;
@@ -536,11 +549,10 @@ int cw_batch_create(const cw_circuit *c, uint32_t batch, int device, cw_batch **
         th = 64;
         while (th < 512 && (uint64_t)th < avg) th <<= 1;
         // many tiles per SM hide latency better than wide CTAs: keep <= ~1024 resident threads per SM
-        // (measured on B200: batch 256 -> 512 threads, 512 -> 256, 1024 -> 128)
         u32 tiles = b->batch_padded >> bt;
-        u32 per_sm = (tiles + 147) / 148;
+        u32 per_sm = (tiles + sms - 1) / sms;
         while (th > 64 && (u32)th * per_sm > 1024) th >>= 1;
-        if (tiles < 148u) th = CW_TAPE_LB;  // fewer tiles than SMs: the widest CTA (wide levels finish in one pass; measured 6.5 vs 7.6 ms at 8 instances)
+        if (tiles < sms) th = CW_TAPE_LB;  // fewer tiles than SMs: the widest CTA (wide levels finish in one pass)
     }
     th = (th + 31) / 32 * 32;
     if (th > CW_TAPE_LB) th = CW_TAPE_LB;
@@ -693,7 +705,7 @@ int cw_batch_run(cw_batch *b) {
     CU(cudaEventRecord(b->ev[0], b->stream));
     {
         size_t total = (size_t)b->batch_padded * (t.n_inputs + 1);
-        u32 grid = (u32)std::min<size_t>((total + 255) / 256, 148 * 8);
+        u32 grid = (u32)std::min<size_t>((total + 255) / 256, device_sms() * 8);
         stage_inputs_kernel<<<grid, 256, 0, b->stream>>>(tp, b->inputs_d, b->slots, b->batch, b->batch_padded, b->bt_log2);
     }
     u32 tiles = b->batch_padded >> b->bt_log2;
@@ -746,7 +758,7 @@ int cw_batch_status(cw_batch *b, int32_t *status) {
 static int expand_rows(cw_batch *b, u32 first, u32 count, uint4 *dst) {
     const Tape &t = b->c->tape;
     if (count == 0) return CW_OK;
-    dim3 grid((u32)std::min<size_t>((t.n_witness + 255) / 256, 148 * 4), std::min<u32>(count, 65535u));
+    dim3 grid((u32)std::min<size_t>((t.n_witness + 255) / 256, device_sms() * 4), std::min<u32>(count, 65535u));
     witness_expand_kernel<<<grid, 256, 0, b->stream>>>(b->store(), b->dt.wloc, (u32)t.n_witness, first, count, dst);
     CU(cudaGetLastError());
     return CW_OK;
@@ -815,7 +827,7 @@ static int ensure_pack_buffers(cw_batch *b, const PackLayout &L) {
 // classes (else the proven one, whose location lists are part of the device tape)
 static int pack_rows(cw_batch *b, const PackLayout &L, u32 first, u32 count, u32 *dst_d, const NarrowPack *np = nullptr) {
     const size_t items = L.n_plane_words + L.n_bit_words + L.u64_loc.size() + L.full_loc.size();
-    dim3 grid((u32)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, 148 * 4)), std::min<u32>(count, 65535u));
+    dim3 grid((u32)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, device_sms() * 4)), std::min<u32>(count, 65535u));
     witness_pack_kernel<<<grid, 256, 0, b->stream>>>(b->store(), np ? np->pk_bit : b->dt.pk_bit, (u32)L.bit_loc.size(),
                                                      np ? np->pk_u64 : b->dt.pk_u64, (u32)L.u64_loc.size(),
                                                      np ? np->pk_full : b->dt.pk_full, (u32)L.full_loc.size(), dst_d, L.words,
@@ -855,7 +867,7 @@ static int observe_classes(cw_batch *b, std::shared_ptr<NarrowPack> prev, std::s
         if ((rc = upload(&cls_d, cls.data(), cls.size() * 4))) { cudaFree(loc_d); return rc; }
         const u32 n_tiles = (b->batch + (1u << b->bt_log2) - 1) >> b->bt_log2;
         const uint64_t items = (uint64_t)loc.size() << b->bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, 148 * 8)), std::min<u32>(n_tiles, 65535u));
+        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         witness_observe_kernel<<<grid, 256, 0, b->stream>>>(b->store(), loc_d, (u32)loc.size(), cls_d);
         cudaError_t e = cudaMemcpyAsync(cls.data(), cls_d, cls.size() * 4, cudaMemcpyDeviceToHost, b->stream);
         if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
@@ -1297,7 +1309,7 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
     const u32 n_tiles = (S.batch + (1u << S.bt_log2) - 1) >> S.bt_log2;
     if (d.n_general) {
         const uint64_t items = (uint64_t)d.n_general << S.bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, 148 * 8)), std::min<u32>(n_tiles, 65535u));
+        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         // long rows: many resident warps (48 registers); short rows: the unspilled build
         const bool lean = env_int("CW_R1CS_LEAN", d.mean_row_terms >= 12 ? 1 : 0) != 0;
         EvalOut eo;
@@ -1322,7 +1334,7 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
         rd.perm = d.perm_small;
         rd.n_rows = d.n_small;
         const uint64_t items = (uint64_t)d.n_small << S.bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, 148 * 8)), std::min<u32>(n_tiles, 65535u));
+        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         R1csSmallDev sg;
         sg.groups = d.sgroups;
         sg.recs = d.srecs;
@@ -1336,7 +1348,7 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
     }
     if (d.n_bool && !eval) {
         const uint64_t items = (uint64_t)d.n_bool << S.bt_log2;
-        dim3 bgrid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, 148 * 8)), std::min<u32>(n_tiles, 65535u));
+        dim3 bgrid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         r1cs_bool_kernel<<<bgrid, 256, 0, stream>>>(d.bool_loc, d.bool_row, d.n_bool, S, fb_d);
     }
     CU(cudaGetLastError());
@@ -1887,7 +1899,7 @@ int cw_fr_batch_op(int prime_id, int op, const uint64_t *a, const uint64_t *b, c
     CU(cudaMalloc((void **)&Rr, n * 32 + 32));
     CU(cudaMalloc((void **)&err, 4));
     CU(cudaMemset(err, 0, 4));
-    u32 grid = (u32)std::min<size_t>((n + 127) / 128, 148 * 16);
+    u32 grid = (u32)std::min<size_t>((n + 127) / 128, device_sms() * 16);
     if (!grid) grid = 1;
     if (prime_id == 0) fr_batch_op_kernel<0><<<grid, 128>>>(op, A, B, C, Rr, n, err, 0u);
     else if (prime_id == 1) fr_batch_op_kernel<1><<<grid, 128>>>(op, A, B, C, Rr, n, err, 1u);

@@ -190,9 +190,9 @@ CW_HD void fr_mont_mul_c(u32 *r, const u32 *a, const u32 *b, const FrParams &P) 
 // PTX carry-chain CIOS on the integer (IMAD) pipe: per outer iteration the 8 low halves and the 8 high
 // halves of a*b[i] are accumulated as two pure carry chains (mad.lo.cc / madc.lo.cc, mad.hi.cc /
 // madc.hi.cc), likewise for m*q, then the accumulator moves down one limb.  39 integer instructions per
-// iteration, 8 iterations, one conditional subtraction.  Same result as fr_mont_mul_c.  MEASURED SLOWER on
-// B200 than the portable form, which nvcc compiles to IMAD.WIDE (both halves of a limb product in one
-// instruction): 43.4 vs 49.5 G modmul/s (scripts/mul_bench.py) - kept behind -DCW_MONT_PTX for reference.
+// iteration, 8 iterations, one conditional subtraction.  Same result as fr_mont_mul_c.  Off by default: the
+// portable form compiles to IMAD.WIDE (both halves of a limb product in one instruction); compare the two with
+// scripts/mul_bench.py - kept behind -DCW_MONT_PTX for reference.
 __device__ __forceinline__ void fr_mont_step(u32 *t, const u32 *a, u32 bi, const FrParams &P) {
     u32 m;
     asm("{\n\t"

@@ -310,8 +310,8 @@ Pool::Pool(int node_hint) : p_(new Impl()) {
         else
             for (size_t k = 0; k < nodes.size(); ++k) use.push_back((int)k);
     }
-    // measured on the 2 x 32-core host of the B200 boxes: 8 threads 246 GB/s, 16 threads 375 GB/s (the memory system's
-    // ceiling for streaming stores), 32 and 64 threads slower and erratic
+    // streaming stores saturate a host's memory system with a few threads per node; many more threads than that
+    // are slower and erratic, so the default stays at half the hardware threads per rank, 4 to 16
     unsigned dflt = std::max(4u, std::min(16u, hw / 2 / ranks));
     unsigned nt = (unsigned)std::max(1, env_int("CW_UNPACK_THREADS", (int)dflt));
     nt = std::min(nt, hw);

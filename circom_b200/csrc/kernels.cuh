@@ -1,4 +1,4 @@
-// sm_100a kernels: tape execution, input staging, witness gather, R1CS check, field batch ops.
+// sm_90a kernels: tape execution, input staging, witness gather, R1CS check, field batch ops.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -22,21 +22,24 @@ __constant__ FrParams c_fr[N_PRIMES_DEV];
 //     uint4 index = (tile * n_slots + slot) * 2 * BT + half * BT + instance_in_tile
 // so a (warp of) thread(s) working on BT instances of one op issues 128-bit loads over
 // BT*16 contiguous bytes per half; with BT = 1 this is the plain 32-byte element (one DRAM sector).
-// sm_100 moves a whole 32-byte element with one instruction (LDG/STG.E.ENL2.256): half the memory
-// instructions and half the L1/L2 requests of a pair of 128-bit accesses.  32-byte alignment required.
+// sm_90's widest global access is 128 bits: a 32-byte element is two adjacent 16-byte accesses, which the
+// two instructions issue back to back into the same 32-byte sector.  32-byte alignment required.
 __device__ __forceinline__ void ldg256(u32 *v, const void *p) {
-    asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
                  : "l"(p)
                  : "memory");
 }
 __device__ __forceinline__ void ldg256_nc(u32 *v, const void *p) {  // data that no thread of the kernel writes
-    asm("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
         : "l"(p));
 }
 __device__ __forceinline__ void stg256(void *p, const u32 *v) {
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]),
+    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};\n\t"
+                 "st.global.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]),
                  "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
                  : "memory");
 }

@@ -1,5 +1,5 @@
 /*
- * circom_b200 — C ABI of the Blackwell (sm_100a) witness-generation and R1CS
+ * circom_b200 — C ABI of the Hopper (sm_90a) witness-generation and R1CS
  * evaluation back end for circom circuits.
  *
  * This is the drop-in boundary a `code_producers/src/cuda_elements` producer

@@ -9,7 +9,7 @@ sys.path.insert(0, ROOT)
 import numpy as np
 
 
-def main(n=512, batch=18944):
+def main(n=512, batch=16896):
     import torch
     from circom_b200.circuit import CircuitDesc
     from circom_b200.witness_calculator import Circuit, Batch, R1cs

@@ -9,7 +9,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from circom_b200 import native  # noqa: E402
 
-n = 148 * 2048 * 4
+n = 132 * 2048 * 4
 iters = 2000
 for prime in (0, 1):
     ms = ctypes.c_float()

@@ -20,7 +20,7 @@ for line in txt.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,6}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
     if m and cur:
         counts[cur][m.group(1)] += 1
-lines = ["SASS summary of circom_b200/libcircom_b200.so (cuobjdump -sass, sm_100a), scripts/sass_summary.py",
+lines = ["SASS summary of circom_b200/libcircom_b200.so (cuobjdump -sass, sm_90a), scripts/sass_summary.py",
          "kernel | instructions | LDG/STG.E.ENL2.256 (one 32-byte element per access) | LDG.128 / STG.128 | LDG.64 | IMAD.WIDE | IMAD | IADD3 | "
          "BAR | UTMALDG/UBLKCP (TMA) | HMMA/UTC*MMA (tensor)"]
 for k, c in counts.items():

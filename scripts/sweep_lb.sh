@@ -1,5 +1,5 @@
 #!/bin/bash
-# occupancy sweep of the tape interpreter: batch = 148 x (CTAs per SM) so that the grid is exactly one
+# occupancy sweep of the tape interpreter: batch = 132 x (CTAs per SM, H100 SXM) so that the grid is exactly one
 # wave, with __launch_bounds__(128, MB) capping registers so that MB CTAs of 128 threads fit per SM
 run() {  # minblocks batch
   echo "== minblocks $1 batch $2 threads 128"
@@ -12,13 +12,13 @@ from circom_b200 import build; build.build(force=True, verbose=True)" 2>&1 | gre
   echo
 }
 build ""
-run 1 1184
+run 1 1056
 build "-DCW_TAPE_LB=128 -DCW_TAPE_MINB=9"
-run 9 1332
+run 9 1188
 build "-DCW_TAPE_LB=128 -DCW_TAPE_MINB=10"
-run 10 1480
+run 10 1320
 build "-DCW_TAPE_LB=128 -DCW_TAPE_MINB=12"
-run 12 1776
+run 12 1584
 build "-DCW_TAPE_LB=128 -DCW_TAPE_MINB=16"
-run 16 2368
+run 16 2112
 build ""

@@ -8,8 +8,11 @@ where the reference tree (and oracle/_ref) is absent.
 
     python tests/golden/make_golden.py
 
-Layout: <name>.json = {"prime", "inputs": [input.json objects], "sha256": [...]};  <name>_<i>.wtns.z = zlib of the
-bytes the reference binary wrote for inputs[i].
+Layout: <name>.json = {"prime", "inputs": [input.json objects], "sha256": [...]} (+ "stdout": what the binary printed
+for inputs[i], for circuits with log() calls);  <name>_<i>.wtns.z = zlib of the bytes the reference binary wrote for
+inputs[i].  cli/all_ops.*: the same for the input files of the command-line calculator's test (JSON numbers that the
+reference sends through a double).  field/field_ops.json: per prime, the sha256 of the compiled reference field library's
+results over the cases of tests/test_oracle_ref.py.
 """
 from __future__ import annotations
 
@@ -33,6 +36,11 @@ NAMES = ["multiplier2", "all_ops", "all_ops_bls", "less_than8", "poseidon2", "in
          "all_ops_gl", "less_than8_gl", "mixed_array_gl",   # goldilocks: the reference's common64 runtime, 8-byte elements
          "sha256compression", "sha256_64_bls",   # the two SHA calculators take ~11 min of g++ each
          "ecdsa_scale_8x132"]                    # the bench circuit (1.2 M constraints): one case, 38 MB -> 1 MB
+
+
+# the input files of tests/test_gpu_circuits.py::test_cli_matches_reference_calculator
+CLI_INPUTS = [{"a": "0x1234567890abcdef1234", "b": "77"}, {"a": "5", "b": "0b101"}, {"a": 123456789, "b": "0o17"},
+              {"a": 9007199254740993, "b": 1e20}, {"a": -5, "b": 3.7}, {"a": 18446744073709551617, "b": 255}]
 
 
 def gen_inputs(name: str, d, rng: random.Random):
@@ -85,28 +93,52 @@ def gen_inputs(name: str, d, rng: random.Random):
     raise KeyError(name)
 
 
+def write_fixture(name: str, calc: str, prime: str, inputs, with_stdout: bool) -> None:
+    shas, outs = [], []
+    with tempfile.TemporaryDirectory() as tmp:
+        for i, inp in enumerate(inputs):
+            jp, wp = os.path.join(tmp, "in.json"), os.path.join(tmp, "out.wtns")
+            json.dump(inp, open(jp, "w"))
+            r = subprocess.run([calc, jp, wp], capture_output=True, text=True)
+            assert r.returncode == 0, (name, i, r.stderr[-400:])
+            raw = open(wp, "rb").read()
+            shas.append(hashlib.sha256(raw).hexdigest())
+            outs.append(r.stdout)
+            open(os.path.join(HERE, "%s_%d.wtns.z" % (name, i)), "wb").write(zlib.compress(raw, 9))
+    meta = {"prime": prime, "inputs": inputs, "sha256": shas}
+    if with_stdout:
+        meta["stdout"] = outs
+    json.dump(meta, open(os.path.join(HERE, name + ".json"), "w"), indent=1)
+    print(name, len(inputs), "cases")
+
+
+def write_field_ops() -> None:
+    from oracle import build_ref
+    from tests.test_oracle_ref import FR_PRIMES, reference_fr_digest, reference_gl_digest
+    build_ref.build_all()
+    digests = {p: reference_fr_digest(p) for p in FR_PRIMES}
+    digests["goldilocks"] = reference_gl_digest()
+    os.makedirs(os.path.join(HERE, "field"), exist_ok=True)
+    json.dump(digests, open(os.path.join(HERE, "field", "field_ops.json"), "w"), indent=1)
+    print("field_ops", len(digests), "primes")
+
+
 def main():
-    names = sys.argv[1:] or NAMES          # `make_golden.py <name>...`: only these fixtures
-    build_calcs.build(names)
+    names = sys.argv[1:] or NAMES + ["cli", "field_ops"]    # `make_golden.py <name>...`: only these fixtures
+    if "field_ops" in names:
+        write_field_ops()
+        names = [n for n in names if n != "field_ops"]
+    build_calcs.build([n for n in names if n != "cli"] + (["all_ops"] if "cli" in names else []))
     for name in names:
-        calc = build_calcs.calc_path(name)
+        calc = build_calcs.calc_path("all_ops" if name == "cli" else name)
         assert os.path.exists(calc) and os.path.exists(calc + ".dat"), "reference calculator %s not built" % name
+        if name == "cli":
+            os.makedirs(os.path.join(HERE, "cli"), exist_ok=True)
+            write_fixture(os.path.join("cli", "all_ops"), calc, "bn128", CLI_INPUTS, False)
+            continue
         d = build_calcs.make_desc(name)
         rng = random.Random(zlib.crc32(name.encode()))
-        inputs = gen_inputs(name, d, rng)
-        shas = []
-        with tempfile.TemporaryDirectory() as tmp:
-            for i, inp in enumerate(inputs):
-                jp, wp = os.path.join(tmp, "in.json"), os.path.join(tmp, "out.wtns")
-                json.dump(inp, open(jp, "w"))
-                r = subprocess.run([calc, jp, wp], capture_output=True, text=True)
-                assert r.returncode == 0, (name, i, r.stderr[-400:])
-                raw = open(wp, "rb").read()
-                shas.append(hashlib.sha256(raw).hexdigest())
-                open(os.path.join(HERE, "%s_%d.wtns.z" % (name, i)), "wb").write(zlib.compress(raw, 9))
-        json.dump({"prime": d.prime, "inputs": inputs, "sha256": shas},
-                  open(os.path.join(HERE, name + ".json"), "w"), indent=1)
-        print(name, len(inputs), "cases")
+        write_fixture(name, calc, d.prime, gen_inputs(name, d, rng), bool(d.strings))
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a kernels, called through the C ABI, against the oracle.
+"""GPU parity tests: the sm_90a kernels, called through the C ABI, against the oracle.
 Bit-exact (integer arithmetic)."""
 import ctypes
 import random

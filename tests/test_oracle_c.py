@@ -1,11 +1,8 @@
 """The C oracle (oracle/cw_oracle.c) is pinned against the python model and against the REAL reference
 runtime: the reference's own main.cpp/calcwit.cpp/fr.cpp linked with the hand-lowered <circuit>.cpp
-(oracle/build_calcs.py) is run as `<bin> input.json out.wtns` and its bytes must equal the oracle's
-witness in .wtns framing (and, on the GPU box, the product's .wtns: tests/test_gpu_parity.py)."""
-import json
-import os
+(oracle/build_calcs.py) was run as `<bin> input.json out.wtns` (tests/golden/make_golden.py) and its bytes must
+equal the oracle's witness in .wtns framing (and, on the GPU, the product's .wtns: tests/test_golden.py)."""
 import random
-import subprocess
 
 import numpy as np
 import pytest
@@ -26,15 +23,6 @@ def wtns_frame(q: int, wit: np.ndarray) -> bytes:
     return (b"wtns" + (2).to_bytes(4, "little") + (2).to_bytes(4, "little") + (1).to_bytes(4, "little") +
             (8 + n8).to_bytes(8, "little") + n8.to_bytes(4, "little") + q.to_bytes(n8, "little") +
             n.to_bytes(4, "little") + (2).to_bytes(4, "little") + (n8 * n).to_bytes(8, "little") + body)
-
-
-def input_json(desc, arr_row) -> dict:
-    obj, k = {}, 0
-    for name, _gid, n in desc.main_inputs():
-        vals = [str(int.from_bytes(arr_row[k + j].tobytes(), "little")) for j in range(n)]
-        obj[name] = vals if n > 1 else vals[0]
-        k += n
-    return obj
 
 
 @pytest.mark.parametrize("prime_id", [0, 1, 7])
@@ -75,51 +63,26 @@ REF_NAMES = ["multiplier2", "all_ops", "all_ops_bls", "less_than8", "poseidon2",
 
 
 @pytest.mark.parametrize("name", REF_NAMES)
-def test_reference_runtime_wtns_equals_oracle(name, tmp_path):
-    calc = build_calcs.calc_path(name)
-    if not (os.path.exists(calc) and os.path.exists(calc + ".dat")):
-        pytest.skip("reference calculator %s not built (needs /root/reference; oracle/build_calcs.py)" % name)
+def test_reference_runtime_wtns_equals_oracle(name):
+    """the bytes the reference calculator wrote for the inputs of its golden fixture (tests/golden/make_golden.py) == the
+    oracle's witness in .wtns framing; with log() calls, what the calculator printed == cw_circuit_format_log of the
+    witness == the evaluator's text"""
+    from tests.test_golden import int_inputs, load
+    meta, raws = load(name)
     d = build_calcs.make_desc(name)
-    rng = np.random.default_rng(11)
-    n_in = d.main.n_in
-    arr = np.zeros((2, n_in, 4), dtype=np.uint64)
-    if name.startswith("ecdsa"):
-        arr[:, :, 0] = rng.integers(0, 2**64, size=(2, n_in), dtype=np.uint64)
-    elif name.startswith("less_than"):
-        arr[:, :, 0] = rng.integers(0, 256, size=(2, n_in), dtype=np.uint64)
-    elif name.startswith("table_lookup"):
-        arr[:, :, :] = rng.integers(0, 2**64, size=(2, n_in, 4), dtype=np.uint64)
-        arr[:, :, 3] &= np.uint64(0x0FFFFFFFFFFFFFFF)
-        arr[:, n_in - 1, :] = 0
-        arr[:, n_in - 1, 0] = rng.integers(0, n_in - 1, size=2, dtype=np.uint64)   # sel: a position of the table
-    elif name.startswith("int_div"):
-        arr[:, 0, 0] = rng.integers(0, 2**32, size=2, dtype=np.uint64)
-        arr[:, 1, 0] = rng.integers(1, 2**20, size=2, dtype=np.uint64)
-    else:
-        arr[:, :, :] = rng.integers(0, 2**64, size=(2, n_in, 4), dtype=np.uint64)
-        arr[:, :, 3] &= np.uint64(0x0FFFFFFFFFFFFFFF)
-        if name.startswith("all_ops"):
-            arr[:, 1, 1:] = 0   # keep b small enough that `a ** (b & 15)` etc. stay cheap
-        if d.prime == "goldilocks":   # values below q = 2^64 - 2^32 + 1
-            arr[:, :, 1:] = 0
-            arr[:, :, 0] &= np.uint64(0x7FFFFFFFFFFFFFFF)
-    o = c_oracle.COracle(d.to_bytes())
-    wit, st = o.run(arr)
+    ins = int_inputs(d, meta["inputs"])
+    wit, st = c_oracle.COracle(d.to_bytes()).run(flat_inputs(d, ins))
     assert not st.any()
-    n_cases = 1 if "8x132" in name else 2
-    for i in range(n_cases):
-        jp, wp = str(tmp_path / "in.json"), str(tmp_path / "o.wtns")
-        json.dump(input_json(d, arr[i]), open(jp, "w"))
-        r = subprocess.run([calc, jp, wp], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-400:]
-        assert open(wp, "rb").read() == wtns_frame(d.q, wit[i])
-        if d.strings:   # log() calls: what the calculator printed = cw_circuit_format_log of the witness, = the evaluator's text
+    for i, raw in enumerate(raws):
+        assert wtns_frame(d.q, wit[i]) == raw, (name, i)
+        if d.strings:
             from circom_b200.witness_calculator import Circuit
             from oracle import ir_eval
+            printed = meta["stdout"][i]
             for o0 in (True, False):
                 c = Circuit(d, host_only=True, o0=o0)
                 w2s = c.witness2signal().astype(np.int64)
-                assert c.format_log(wit[i][w2s]) == r.stdout
+                assert c.format_log(wit[i][w2s]) == printed
             ir_eval.LOG_SINK.clear()
-            evaluate(d, {k: (int(v) if not isinstance(v, list) else [int(x) for x in v]) for k, v in input_json(d, arr[i]).items()})
-            assert "".join(ir_eval.LOG_SINK) == r.stdout and r.stdout.count("\n") == 4
+            evaluate(d, ins[i])
+            assert "".join(ir_eval.LOG_SINK) == printed and printed.count("\n") == 4

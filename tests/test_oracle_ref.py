@@ -1,7 +1,12 @@
 """The oracle is pinned against the compiled REFERENCE field library (oracle/_ref/libfr_<prime>.so,
 the reference's own generic/fr.cpp) over every operator and operand representation, and against
 the few worked values the reference tree contains (there are no golden vectors in its tests:
-SURVEY.md section 8(c))."""
+SURVEY.md section 8(c)).  The library's results for the fixed, seeded cases below are stored as one
+digest per prime (tests/golden/field/field_ops.json, written by tests/golden/make_golden.py), so the model is
+pinned where oracle/_ref is not built; where it is, every value is compared as well."""
+import ctypes
+import hashlib
+import json
 import os
 import random
 
@@ -10,12 +15,15 @@ import pytest
 from oracle.field_model import Field, OPS, OP_NAMES, PRIMES
 from tests.util import edge_values, rand_operand
 
-REF_OK = os.path.exists(os.path.join(os.path.dirname(__file__), "..", "oracle", "_ref", "libfr_bn128.so")) or \
-    os.path.isdir("/root/reference")
-needs_ref = pytest.mark.skipif(not REF_OK, reason="oracle/_ref not built and no reference tree")
+REF_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "_ref")
+REF_OK = os.path.exists(os.path.join(REF_DIR, "libfr_bn128.so"))
+GL_OK = os.path.exists(os.path.join(REF_DIR, "libfr_goldilocks.so"))
+needs_ref = pytest.mark.skipif(not REF_OK, reason="oracle/_ref not built")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "field", "field_ops.json")
+FR_PRIMES = ["bn128", "bls12381", "grumpkin", "pallas", "vesta", "secq256r1", "bls12377"]
 
 
-def _reps(R, v, q):
+def _reps(v, q):
     out = [("long", v), ("mont", v)]
     sv = v if v < 2**31 else (v - q if q - v <= 2**31 else None)
     if sv is not None:
@@ -23,15 +31,11 @@ def _reps(R, v, q):
     return out
 
 
-@needs_ref
-@pytest.mark.parametrize("prime", ["bn128", "bls12381", "grumpkin", "pallas", "vesta", "secq256r1", "bls12377"])
-def test_model_matches_reference_fr(prime):
-    from oracle.ref_fr import RefFr
-    F, R = Field(prime), RefFr(prime)
-    q = F.q
+def fr_cases(prime):
+    """(op, a, b, [(representation of a, its value, representation of b, its value)]) in a fixed order"""
+    q = PRIMES[prime]
     rng = random.Random(1234)
     edges = edge_values(q)
-    n = 0
     for it in range(700 if prime in ("bn128", "bls12381") else 250):
         a, b = rand_operand(rng, q, edges), rand_operand(rng, q, edges)
         if rng.random() < 0.25:
@@ -41,52 +45,100 @@ def test_model_matches_reference_fr(prime):
                 continue
             if op == OPS["POW"] and it % 10:
                 continue
-            exp = F.apply(op, a, b)
-            for ra, va in _reps(R, a, q):
-                for rb, vb in _reps(R, b, q):
-                    got = R.apply(op, R.make(va, ra), R.make(vb, rb))
-                    n += 1
-                    assert got == exp, (prime, OP_NAMES[op], ra, rb, hex(a), hex(b), hex(got), hex(exp))
+            yield op, a, b, [(ra, va, rb, vb) for ra, va in _reps(a, q) for rb, vb in _reps(b, q)]
+
+
+def reference_fr_digest(prime) -> str:
+    """sha256 over the reference library's results of fr_cases(prime), 32 little-endian bytes each"""
+    from oracle.ref_fr import RefFr
+    R, h = RefFr(prime), hashlib.sha256()
+    for op, a, b, reps in fr_cases(prime):
+        for ra, va, rb, vb in reps:
+            h.update(R.apply(op, R.make(va, ra), R.make(vb, rb)).to_bytes(32, "little"))
+    return h.hexdigest()
+
+
+@pytest.mark.parametrize("prime", FR_PRIMES)
+def test_model_matches_reference_fr(prime):
+    from oracle.ref_fr import RefFr
+    F = Field(prime)
+    R = RefFr(prime) if REF_OK else None
+    h, n = hashlib.sha256(), 0
+    for op, a, b, reps in fr_cases(prime):
+        exp = F.apply(op, a, b)
+        for ra, va, rb, vb in reps:
+            if R is not None:
+                got = R.apply(op, R.make(va, ra), R.make(vb, rb))
+                assert got == exp, (prime, OP_NAMES[op], ra, rb, hex(a), hex(b), hex(got), hex(exp))
+            h.update(exp.to_bytes(32, "little"))
+            n += 1
     assert n > 15000
+    assert h.hexdigest() == json.load(open(GOLDEN))[prime]
 
 
-@needs_ref
-def test_model_matches_reference_goldilocks():
-    """goldilocks has a field library of its own in the reference (c_elements/goldilocks/fr.hpp: plain uint64_t values,
-    no Montgomery form, no short / long tags); the same python model with q = 2^64 - 2^32 + 1 must describe it, value
-    for value: shifts with their 64-bit truncation (:166-195), the bit operators with one conditional subtraction
-    (:255-270), comparisons on the signed view (:197-239), inv(0) = 0 (:84-106), Fr_toInt (:23-26)."""
-    import ctypes
-    from oracle import build_ref
-    lib = ctypes.CDLL(build_ref.build_goldilocks())
-    lib.gl_apply.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]
-    lib.gl_is_true.argtypes = [ctypes.c_uint64]
-    F = Field("goldilocks")
-    q = F.q
-    assert q == 2**64 - 2**32 + 1 and F.qbits == 64 and F.mask == 2**64 - 1
+def gl_cases():
+    q = PRIMES["goldilocks"]
     rng = random.Random(4321)
     edges = edge_values(q) + [q - 63, q - 65, 2**63, 2**63 + 1, 2**32 * (2**32 - 1), 0xFFFFFFFF, 0xFFFFFFFF00000000 % q]
-    n = 0
     for it in range(6000):
         a, b = rand_operand(rng, q, edges), rand_operand(rng, q, edges)
         if rng.random() < 0.3:
             b = rng.randrange(300)
         for op in list(range(1, 24)) + [28]:
-            r = ctypes.c_uint64(0)
-            rc = lib.gl_apply(op, a, b, ctypes.byref(r))
-            if op in (OPS["IDIV"], OPS["MOD"]) and b == 0:
-                assert rc == 1          # the reference process dies of SIGFPE there; the model raises
-                continue
-            assert rc == 0
-            exp = F.inv(a) if op == 28 else F.apply(op, a, b)
-            n += 1
-            assert r.value == exp, (OP_NAMES.get(op, op), hex(a), hex(b), hex(r.value), hex(exp))
-        assert lib.gl_is_true(a) == int(a != 0)
-    assert n > 100000
-    # Fr_toInt: the signed view, truncated to int (goldilocks/fr.hpp:23-26)
+            yield op, a, b
+
+
+def _gl_record(rc: int, value: int) -> bytes:
+    return bytes([rc]) + (value.to_bytes(8, "little") if rc == 0 else b"")
+
+
+def _gl_lib():
+    from oracle import build_ref
+    lib = ctypes.CDLL(build_ref.build_goldilocks())
+    lib.gl_apply.argtypes = [ctypes.c_int, ctypes.c_uint64, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]
+    lib.gl_is_true.argtypes = [ctypes.c_uint64]
     lib.gl_to_int.argtypes = [ctypes.c_uint64]
-    for v in (0, 1, 5, 2**31 - 1, q - 1, q - 7, q - 2**31):
-        assert lib.gl_to_int(v) == (v if v <= F.half else v - q)
+    return lib
+
+
+def reference_gl_digest() -> str:
+    """sha256 over the reference goldilocks header's (status, result) of gl_cases()"""
+    lib, h = _gl_lib(), hashlib.sha256()
+    for op, a, b in gl_cases():
+        r = ctypes.c_uint64(0)
+        rc = lib.gl_apply(op, a, b, ctypes.byref(r))
+        h.update(_gl_record(rc, r.value))
+    return h.hexdigest()
+
+
+def test_model_matches_reference_goldilocks():
+    """goldilocks has a field library of its own in the reference (c_elements/goldilocks/fr.hpp: plain uint64_t values,
+    no Montgomery form, no short / long tags); the same python model with q = 2^64 - 2^32 + 1 must describe it, value
+    for value: shifts with their 64-bit truncation (:166-195), the bit operators with one conditional subtraction
+    (:255-270), comparisons on the signed view (:197-239), inv(0) = 0 (:84-106), Fr_toInt (:23-26)."""
+    lib = _gl_lib() if GL_OK else None
+    F = Field("goldilocks")
+    q = F.q
+    assert q == 2**64 - 2**32 + 1 and F.qbits == 64 and F.mask == 2**64 - 1
+    h, n = hashlib.sha256(), 0
+    for op, a, b in gl_cases():
+        if op in (OPS["IDIV"], OPS["MOD"]) and b == 0:
+            rc, exp = 1, 0          # the reference process dies of SIGFPE there; the model raises
+        else:
+            rc, exp = 0, (F.inv(a) if op == 28 else F.apply(op, a, b))
+            n += 1
+        if lib is not None:
+            r = ctypes.c_uint64(0)
+            got = lib.gl_apply(op, a, b, ctypes.byref(r))
+            assert got == rc and (rc or r.value == exp), (OP_NAMES.get(op, op), hex(a), hex(b), hex(r.value), hex(exp))
+            if op == 28:
+                assert lib.gl_is_true(a) == int(a != 0)
+        h.update(_gl_record(rc, exp))
+    assert n > 100000
+    assert h.hexdigest() == json.load(open(GOLDEN))["goldilocks"]
+    if lib is not None:   # Fr_toInt: the signed view, truncated to int (goldilocks/fr.hpp:23-26)
+        for v in (0, 1, 5, 2**31 - 1, q - 1, q - 7, q - 2**31):
+            assert lib.gl_to_int(v) == (v if v <= F.half else v - q)
 
 
 @needs_ref

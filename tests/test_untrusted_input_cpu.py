@@ -150,7 +150,7 @@ def test_cli_rejects_pathological_json(tmp_path):
 def test_cli_directory_of_inputs(tmp_path):
     """`circom_cuda_witness circuit.cb2c <directory of *.json> <output directory>`: one input per file, taken in name order,
     other files ignored; an empty directory is an error; a malformed file is reported.  (Without a GPU the run stops where
-    the batch is created - after every file has been read and parsed; on a B200 it writes <name>.wtns per input.)"""
+    the batch is created - after every file has been read and parsed; on a GPU it writes <name>.wtns per input.)"""
     import json
     import os
     import subprocess
