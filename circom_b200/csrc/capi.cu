@@ -482,6 +482,12 @@ int cw_circuit_slot_census(const cw_circuit *c, uint64_t out[4]) {
     return CW_OK;
 }
 
+int cw_circuit_width_census(const cw_circuit *c, uint64_t out[256]) {
+    if (!c || !out) return fail(CW_EINVAL, "null argument");
+    memcpy(out, c->tape.width_census, sizeof(c->tape.width_census));
+    return CW_OK;
+}
+
 int cw_circuit_witness2signal(const cw_circuit *c, uint64_t *out) {
     if (!c || !out) return fail(CW_EINVAL, "null argument");
     memcpy(out, c->tape.witness2signal.data(), c->tape.witness2signal.size() * 8);

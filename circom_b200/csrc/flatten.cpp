@@ -117,6 +117,9 @@ struct Val {
 
 // device-only opcodes (kernels.cuh / fr_device.cuh)
 enum { DOP_BITS = 29, DOP_ASSERT_BOOL = 30, DOP_MULSMALL = 31, DOP_BITSIP = 32, DOP_ASSERT_FITS = 33 };
+// width-classed forms (fr_device.cuh OP_ADDI ...): chosen when the tape word is written, from the static widths
+enum { DOP_ADDI = 48, DOP_SHRK = 49, DOP_SHLK = 50, DOP_ADDI_H = 52, DOP_MULI_Q = 53, DOP_MULI_H = 54, DOP_SHRK_H = 55,
+       DOP_SHLK_H = 56 };
 inline bool c_is_immediate(uint32_t opcode) {
     return opcode == CW_OP_ASSERT || opcode == CW_OP_ASSERT_EQ || opcode == DOP_BITS || opcode == DOP_ASSERT_BOOL ||
            opcode == DOP_BITSIP || opcode == DOP_ASSERT_FITS;
@@ -1647,10 +1650,63 @@ struct Lowerer {
         T.level_start.assign(max_level + 1, 0);
         T.n_mul_ops = 0;
         uint32_t prev_level = 0;
+        // Width classes.  Most operators of limb arithmetic work on values the range analysis bounds far below q (64-bit
+        // limbs, their products and sums, the splits at 2^64).  Such an operator IS the integer operation: it gets a form
+        // that skips the reduction, the mask or the shift-direction test, and whose operands below 2^128 are read as the
+        // low 16 bytes of their slots.  Each form is exact under the bounds checked here; the result is stored at full
+        // width (the high limbs it writes are zero), so no reader depends on how its operand was produced.
+        const bool narrow_on = !(flags & (CW_FLAG_NO_NARROW | CW_FLAG_NO_PEEPHOLE));
+        auto opd_bits = [&](uint32_t o) -> uint32_t {   // static width of an operand: provisional slot or constant
+            if (o == NO_SLOT) return 0;
+            if (o & OPERAND_CONST) return (uint32_t)u256_bitlen(consts[o & 0x7FFFFFFFu]);
+            return o < slot_bits.size() ? slot_bits[o] : 256u;
+        };
+        auto const_amount = [&](uint32_t o, uint32_t &k) {   // a constant operand below qbits (a shift amount)
+            if (o == NO_SLOT || !(o & OPERAND_CONST)) return false;
+            const U256 &c = consts[o & 0x7FFFFFFFu];
+            if (c.v[1] | c.v[2] | c.v[3] || c.v[0] >= qb()) return false;
+            k = (uint32_t)c.v[0];
+            return true;
+        };
+        auto narrow_opcode = [&](uint32_t i) -> uint32_t {
+            const uint32_t *o = &pops[(size_t)i * 4];
+            if (!narrow_on) return o[0];
+            // a result width below 256 is only ever recorded for a canonical value: the operator ran in canonical form
+            const uint32_t rb = slot_bits[n_pre + i], ba = opd_bits(o[1]), bb = opd_bits(o[2]), lim = qb() - 1;
+            uint32_t k;
+            switch (o[0]) {
+                case CW_OP_ADD:
+                    if (rb >= 256 || std::max(ba, bb) + 1 > lim) return o[0];
+                    return std::max(ba, bb) + 1 <= 128 ? DOP_ADDI_H : DOP_ADDI;
+                case DOP_MULSMALL:   // (the lowering emits it only for ba + bb <= qbits - 1)
+                    if (ba <= 64 && bb <= 64) return DOP_MULI_Q;
+                    if (ba <= 128 && bb <= 128) return DOP_MULI_H;
+                    return o[0];
+                case CW_OP_SHR:
+                    if (!const_amount(o[2], k)) return o[0];
+                    return ba <= 128 ? DOP_SHRK_H : DOP_SHRK;
+                case CW_OP_SHL:
+                    if (!const_amount(o[2], k) || ba + k > lim) return o[0];
+                    return ba <= 128 ? DOP_SHLK_H : DOP_SHLK;
+                default: return o[0];
+            }
+        };
+        for (uint64_t &x : T.width_census) x = 0;
+        // per tape word (a run of bit extractions counts once, with the width of its source)
+        auto census = [&](uint32_t i, uint32_t opcode) {   // widest of the result and the slot operands (constants do not count)
+            const uint32_t *o = &pops[(size_t)i * 4];
+            uint32_t w = is_assert_op(o[0]) ? 0u : slot_bits[n_pre + i];
+            for (int k = 1; k <= 3; ++k) {
+                if (k == 3 && c_is_immediate(o[0])) break;
+                if (o[k] != NO_SLOT && !(o[k] & OPERAND_CONST)) w = std::max(w, opd_bits(o[k]));
+            }
+            T.width_census[4 * (opcode & 63u) + (w <= 64 ? 0 : w <= 128 ? 1 : w <= 192 ? 2 : 3)]++;
+        };
         // one operator as a tape word; operands that are fused producers read an accumulator
         auto word = [&](uint32_t i, uint32_t dstfield, int acc_a, int acc_b, uint32_t d[4]) {
             const uint32_t *o = &pops[(size_t)i * 4];
-            d[0] = o[0] | (dstfield << 8);  // opcode in bits 0-7, destination in bits 8-31
+            const uint32_t opcode = o[0] == 45 ? o[0] : narrow_opcode(i);
+            d[0] = opcode | (dstfield << 8);  // opcode in bits 0-7, destination in bits 8-31
             if (o[0] == 45) {
                 uint32_t n = pcalls[o[1] + 1];
                 d[1] = (uint32_t)T.call_tab.size();
@@ -1690,6 +1746,7 @@ struct Lowerer {
             else if (kb != NO_SLOT) { emit_sub(kb, target); acc_b = target; }
             uint32_t d[4];
             word(i, DST_ACC + (uint32_t)target, acc_a, acc_b, d);
+            census(i, d[0] & 0xFFu);
             T.ops.insert(T.ops.end(), d, d + 4);
             if (pops[(size_t)i * 4] == CW_OP_MUL) ++T.n_mul_ops;
         };
@@ -1717,6 +1774,7 @@ struct Lowerer {
                         }
                     }
                 }
+                if (o[0] != 45) census(i, d[0] & 0xFFu);
                 T.items.push_back((uint32_t)(T.ops.size() / 4));
                 T.ops.insert(T.ops.end(), d, d + 4);
             } else {
@@ -1731,6 +1789,7 @@ struct Lowerer {
                 } else if (ka != NO_SLOT) { emit_sub(ka, 0); acc_a = 0; }
                 else { emit_sub(kb, 0); acc_b = 0; }
                 word(i, dst, acc_a, acc_b, d);
+                census(i, d[0] & 0xFFu);
                 T.ops.insert(T.ops.end(), d, d + 4);
             }
             prev_level = lvl;
@@ -2002,7 +2061,7 @@ struct BlobR {
         p += n;
     }
 };
-constexpr uint32_t BLOB_VERSION = 6;
+constexpr uint32_t BLOB_VERSION = 7;   // 7: width-classed opcodes, width census
 }  // namespace
 
 void serialize_tape(const Tape &t, std::vector<uint8_t> &out) {
@@ -2020,6 +2079,7 @@ void serialize_tape(const Tape &t, std::vector<uint8_t> &out) {
     w.vec(t.ops); w.vec(t.items); w.vec(t.level_start); w.vec(t.consts); w.vec(t.dat_consts); w.vec(t.witness_slot); w.vec(t.input_slot);
     w.vec(t.pk_bit_wire); w.vec(t.pk_u64_wire); w.vec(t.pk_full_wire); w.vec(t.wit_class); w.vec(t.wit_bits);
     w.vec(t.fn_code); w.vec(t.fn_info); w.vec(t.call_tab); w.vec(t.witness2signal);
+    w.raw(t.width_census, sizeof(t.width_census));
     w.pod<uint64_t>(t.inputs.size());
     for (const InputInfo &in : t.inputs) {
         w.str(in.name);
@@ -2058,6 +2118,7 @@ void deserialize_tape(const uint8_t *data, size_t len, Tape &t) {
     r.vec(t.ops); r.vec(t.items); r.vec(t.level_start); r.vec(t.consts); r.vec(t.dat_consts); r.vec(t.witness_slot); r.vec(t.input_slot);
     r.vec(t.pk_bit_wire); r.vec(t.pk_u64_wire); r.vec(t.pk_full_wire); r.vec(t.wit_class); r.vec(t.wit_bits);
     r.vec(t.fn_code); r.vec(t.fn_info); r.vec(t.call_tab); r.vec(t.witness2signal);
+    r.raw(t.width_census, sizeof(t.width_census));
     uint64_t n_in;
     r.pod(n_in);
     if (n_in > len) throw std::runtime_error("lowered-circuit blob: bad length");

@@ -650,6 +650,20 @@ enum {
     OP_BITSIP = 32,       // a & ((2^len - 1) << lo), imm = lo | len << 8  (sum of adjacent bit fields)
     OP_ASSERT_FITS = 33   // a < 2^m, m = b[0]  (recomposition check of a bit decomposition)
 };
+// Width-classed forms (flatten.cpp, from the range analysis): the lowering proves the canonical operands and the result
+// small enough that the field operation IS the integer one, and the operator reads only the limbs the bounds allow.
+// Opcodes from OP_NARROW_HALF on read operands below 2^128: the interpreter loads only the low 16 bytes of their slots.
+enum {
+    OP_ADDI = 48,     // a + b, the sum proven below 2^(qbits-1) < q: no reduction
+    OP_SHRK = 49,     // a >> k, k = b[0] < qbits (a plain right shift: no "negative" amount)
+    OP_SHLK = 50,     // a << k, k = b[0], the result proven below 2^(qbits-1): no mask, no wrap
+    OP_NARROW_HALF = 52,
+    OP_ADDI_H = 52,   // OP_ADDI on operands and result below 2^128: 4 limbs
+    OP_MULI_Q = 53,   // a * b with a, b < 2^64: 4 limb products (OP_MULSMALL takes 36)
+    OP_MULI_H = 54,   // a * b with a, b < 2^128: 16 limb products
+    OP_SHRK_H = 55,   // OP_SHRK on a < 2^128
+    OP_SHLK_H = 56    // OP_SHLK on a < 2^128
+};
 
 // low 256 bits of the integer product (36 limb products instead of CIOS' 128)
 CW_HD void u256_mul_lo(u32 *r, const u32 *a, const u32 *b) {
@@ -667,6 +681,51 @@ CW_HD void u256_mul_lo(u32 *r, const u32 *a, const u32 *b) {
         }
     }
     u256_set(r, t);
+}
+// r = a * b for a, b < 2^(32 N): the full 2N-limb product of the low N limbs, r[2N..7] = 0 (N = 2 or 4)
+template <int N>
+CW_HD void u256_mul_narrow(u32 *r, const u32 *a, const u32 *b) {
+    u32 t[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t[i] = 0;
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        u64 c = 0;
+#pragma unroll
+        for (int j = 0; j < N; ++j) {
+            c += (u64)a[j] * b[i] + t[i + j];
+            t[i + j] = (u32)c;
+            c >>= 32;
+        }
+        t[i + N] = (u32)c;
+    }
+    u256_set(r, t);
+}
+// r = a + b over the low 4 limbs (a + b < 2^128), r[4..7] = 0
+CW_HD void u128_add(u32 *r, const u32 *a, const u32 *b) {
+#if defined(__CUDA_ARCH__)
+    u32 r0, r1, r2, r3;
+    asm("add.cc.u32 %0, %4, %8;\n\t"
+        "addc.cc.u32 %1, %5, %9;\n\t"
+        "addc.cc.u32 %2, %6, %10;\n\t"
+        "addc.u32 %3, %7, %11;"
+        : "=&r"(r0), "=&r"(r1), "=&r"(r2), "=&r"(r3)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]), "r"(b[2]), "r"(b[3]));
+    r[0] = r0; r[1] = r1; r[2] = r2; r[3] = r3;
+#else
+    u64 c = 0;
+    for (int i = 0; i < 4; ++i) {
+        c += (u64)a[i] + b[i];
+        r[i] = (u32)c;
+        c >>= 32;
+    }
+#endif
+    r[4] = r[5] = r[6] = r[7] = 0;
+}
+// the low 4 limbs of a, zero-extended (the operand of an _H operator: its upper limbs are never read)
+CW_HD void u256_low_half(u32 *r, const u32 *a) {
+    r[0] = a[0]; r[1] = a[1]; r[2] = a[2]; r[3] = a[3];
+    r[4] = r[5] = r[6] = r[7] = 0;
 }
 CW_HD void u256_bits(u32 *r, const u32 *a, u32 imm) {
     u32 k = imm & 0xFFFFu, m = (imm >> 16) & 0xFFu;
@@ -755,6 +814,14 @@ CW_HD void fr_exec_t(u32 opcode, u32 *r, const u32 *a, const u32 *b, u32 imm, co
             fr_mask_wrap(r, P);
             break;
         case OP_COPY: u256_set(r, a); break;
+        case OP_ADDI: u256_add(r, a, b); break;
+        case OP_SHRK: u256_shr(r, a, b[0]); break;
+        case OP_SHLK: u256_shl(r, a, b[0]); break;
+        case OP_ADDI_H: u128_add(r, a, b); break;
+        case OP_MULI_Q: u256_mul_narrow<2>(r, a, b); break;
+        case OP_MULI_H: u256_mul_narrow<4>(r, a, b); break;
+        case OP_SHRK_H: { u32 t[8]; u256_low_half(t, a); u256_shr(r, t, b[0]); break; }
+        case OP_SHLK_H: { u32 t[8]; u256_low_half(t, a); u256_shl(r, t, b[0]); break; }
         default: u256_set_u32(r, 0); break;
     }
 }

@@ -24,6 +24,8 @@ __constant__ FrParams c_fr[N_PRIMES_DEV];
 // BT*16 contiguous bytes per half; with BT = 1 this is the plain 32-byte element (one DRAM sector).
 // sm_90's widest global access is 128 bits: a 32-byte element is two adjacent 16-byte accesses, which the
 // two instructions issue back to back into the same 32-byte sector.  32-byte alignment required.
+// Every store writes the whole slot (a value below 2^128 with zero high limbs); the width-classed operators
+// (opcode >= OP_NARROW_HALF) read only the low half of operands the lowering proved below 2^128.
 __device__ __forceinline__ void ldg256(u32 *v, const void *p) {
     asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
                  "ld.global.v4.b32 {%4,%5,%6,%7}, [%8+16];"
@@ -83,15 +85,35 @@ __device__ __forceinline__ u32 load_plane_bit(const u32 *__restrict__ plane_base
     return (plane_base[((size_t)(pos >> 5) << bt_log2) + li] >> (pos & 31u)) & 1u;
 }
 
-// operand of a tape op: constant-table entry, a bit of the bit plane, or a value slot
+// the low 16 bytes of a slot (a value the lowering proved below 2^128), zero-extended: one 128-bit access instead of two
+__device__ __forceinline__ void load_slot_low(u32 *v, const uint4 *__restrict__ tile_base, u32 slot, u32 bt_log2, u32 inst) {
+    uint4 lo;
+    if (bt_log2 == 0) {
+        asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(lo.x), "=r"(lo.y), "=r"(lo.z), "=r"(lo.w)
+                     : "l"(tile_base + ((size_t)slot << 1)) : "memory");
+    } else {
+        lo = tile_base[((size_t)slot << (bt_log2 + 1)) + inst];
+    }
+    v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w;
+    v[4] = v[5] = v[6] = v[7] = 0;
+}
+
+// operand of a tape op: constant-table entry, a bit of the bit plane, or a value slot.  half: the operator reads operands
+// below 2^128 (opcode >= OP_NARROW_HALF) - only the low half of a slot or constant is fetched.
 template <bool BP>
 __device__ __forceinline__ void load_operand(u32 *v, u32 operand, const uint4 *__restrict__ tile_base,
                                              const u32 *__restrict__ plane_base, const uint4 *__restrict__ consts,
-                                             u32 bt_log2, u32 li) {
+                                             u32 bt_log2, u32 li, bool half = false) {
     if (operand & OPD_CONST) {
-        load_const(v, consts, operand & 0x7FFFFFFFu);
+        if (half) {
+            const uint4 lo = __ldg(&consts[2 * (size_t)(operand & 0x7FFFFFFFu)]);
+            v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w;
+            v[4] = v[5] = v[6] = v[7] = 0;
+        } else load_const(v, consts, operand & 0x7FFFFFFFu);
     } else if (BP && (operand & OPD_BIT)) {
         u256_set_u32(v, load_plane_bit(plane_base, operand & OPD_BITPOS, bt_log2, li));
+    } else if (half) {
+        load_slot_low(v, tile_base, operand & OPD_SLOT, bt_log2, li);
     } else {
         load_slot(v, tile_base, operand & OPD_SLOT, bt_log2, li);
     }
@@ -324,14 +346,15 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 } else r[0] = (u32)window & (m >= 32u ? 0xFFFFFFFFu : ((1u << m) - 1u));
             } else {
                 u32 a[8], b[8];
+                const bool half = opcode >= OP_NARROW_HALF;   // width-classed operators on operands below 2^128
                 if (FUSED && !(opw.y & OPD_CONST) && (opw.y & OPD_ACC)) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) a[i] = (opw.y & 1u) ? acc1[i] : acc0[i];
-                } else load_operand<BP>(a, opw.y, base, plane_base, tp.consts, bt_log2, li);
+                } else load_operand<BP>(a, opw.y, base, plane_base, tp.consts, bt_log2, li, half);
                 if (FUSED && !(opw.z & OPD_CONST) && (opw.z & OPD_ACC)) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) b[i] = (opw.z & 1u) ? acc1[i] : acc0[i];
-                } else load_operand<BP>(b, opw.z, base, plane_base, tp.consts, bt_log2, li);
+                } else load_operand<BP>(b, opw.z, base, plane_base, tp.consts, bt_log2, li, half);
                 if (opcode == OP_SELECT) {
                     u32 c[8];
                     load_operand<BP>(c, opw.w, base, plane_base, tp.consts, bt_log2, li);

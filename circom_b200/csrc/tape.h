@@ -54,6 +54,8 @@ struct Tape {
     uint64_t n_signals = 0, n_witness = 0, n_inputs = 0, n_outputs = 0, n_components = 0;
     uint64_t n_ir_ops = 0, n_mul_ops = 0, n_conv_ops = 0, max_level_width = 0, n_asserts = 0;
     uint64_t slot_census[4] = {0, 0, 0, 0};  // value slots by static width: 1 bit, <= 32, <= 64 bits, wider
+    // operators by emitted opcode (< 64) and the static width of their result and slot operands: <= 64, 128, 192 bits, wider
+    uint64_t width_census[64 * 4] = {};
     uint64_t n_slot_operands = 0;  // operand reads of slots
     uint64_t n_stored = 0;         // values that reach the value store (slots / plane words written): n_values minus the fused ones
     uint64_t n_values = 0;         // values the tape computes per instance (every destination, each bit of a run)

@@ -15,6 +15,7 @@ CW_OK, CW_EINVAL, CW_EIO, CW_EFORMAT, CW_ECUDA, CW_ENOTFOUND, CW_ESTATE, CW_ENOD
 CW_FLAG_NO_ASSERTS, CW_FLAG_HOST_ONLY, CW_FLAG_O0, CW_FLAG_NO_PEEPHOLE, CW_FLAG_BITPLANE, CW_FLAG_REUSE = 1, 2, 4, 8, 16, 32
 CW_FLAG_COMPACT = CW_FLAG_BITPLANE | CW_FLAG_REUSE
 CW_FLAG_FUSE = 64
+CW_FLAG_NO_NARROW = 128
 
 
 class CwError(RuntimeError):
@@ -61,6 +62,7 @@ def _load() -> ctypes.CDLL:
         "cw_circuit_tape": (c_int, [P, c_void_p, c_void_p, c_void_p]),
         "cw_circuit_tape_items": (c_int, [P, c_void_p]),
         "cw_circuit_slot_census": (c_int, [P, POINTER(c_uint64)]),
+        "cw_circuit_width_census": (c_int, [P, POINTER(c_uint64)]),
         "cw_circuit_witness2signal": (c_int, [P, c_void_p]),
         "cw_circuit_write_dat": (c_int, [P, c_char_p]),
         "cw_circuit_write_sym": (c_int, [P, c_char_p]),

@@ -57,6 +57,8 @@ extern "C" {
 #define CW_FLAG_FUSE 64u       /* single-use values are evaluated inside their reader's work item (two accumulator registers) instead
                                   of travelling through the value store: half the levels, 30 % fewer stores; pays only for large
                                   batches (measured: DESIGN.md section 7) */
+#define CW_FLAG_NO_NARROW 128u /* emit every operator at full width: no width-classed forms (plain integer ADD / MULSMALL / shifts
+                                  that read only the limbs the range analysis allows; for A/B comparisons) */
 #define CW_FLAG_COMPACT (CW_FLAG_BITPLANE | CW_FLAG_REUSE) /* the compact value store: what cw_batch_* runs best on */
 #define CW_FLAG_O0 4u         /* --O0: keep every signal in the witness and every `signal = signal` constraint */
 
@@ -136,6 +138,10 @@ int cw_circuit_tape_items(const cw_circuit *c, uint32_t *items);
 /* value slots of one instance by the width the lowering's range analysis proves: out[0] one bit, out[1] <= 32 bits,
  * out[2] <= 64 bits, out[3] wider (today every slot is a 32-byte element; the census sizes a narrow-slot layout) */
 int cw_circuit_slot_census(const cw_circuit *c, uint64_t out[4]);
+/* operators of the tape by opcode as emitted (out[4 * opcode + class], opcodes 0-63) and by the static width class of the
+ * widest of their result and slot operands (constants do not count): class 0 <= 64 bits, 1 <= 128, 2 <= 192, 3 wider.
+ * Opcodes 48-56 are the width-classed forms (fr_device.cuh); CW_FLAG_NO_NARROW leaves them out. */
+int cw_circuit_width_census(const cw_circuit *c, uint64_t out[256]);
 /* the circuit's functions (FunctionCodeInfo, function.rs:9-20) as lowered: *n = their number; info (may be NULL) receives 4
  * words per function: {code offset, instructions, registers of a call frame after register allocation, parameters} */
 int cw_circuit_functions(const cw_circuit *c, uint32_t *n, uint32_t *info);
