@@ -264,17 +264,8 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
     u32 *plane_base = BP ? plane + (((size_t)tile * tp.n_bitwords) << bt_log2) : nullptr;
     u32 lb = tp.level_start[0];
     u32 le = tp.n_levels ? tp.level_start[1] : lb;
-    // the first tape word of a thread's first work item of the next level is fetched before the barrier of the
-    // current one, taking the memory round trips of the item table and the tape off the per-level critical path
-    uint4 pre = make_uint4(0, 0, 0, 0);
-    u32 pre_g0 = 0, pre_g1 = 0;
-    if (threadIdx.x < ((le - lb) << bt_log2)) {
-        if (FUSED) {
-            pre_g0 = __ldg(&tp.items[lb + (threadIdx.x >> bt_log2)]);
-            pre_g1 = __ldg(&tp.items[lb + (threadIdx.x >> bt_log2) + 1]);
-            pre = __ldg(&tp.heads[lb + (threadIdx.x >> bt_log2)]);
-        } else pre = __ldg(&tp.ops[lb + (threadIdx.x >> bt_log2)]);
-    }
+    // (A thread's first item of a level is fetched like the others, not before the barrier: held in registers, its head
+    // word and bounds would stay live through every item of the level and make the fused build spill - DESIGN §7.)
     for (u32 l = 0; l < tp.n_levels; ++l) {
         // Calls are the last work items of their level (the items of a level are sorted by opcode, CALL is the largest) and
         // run in a loop of their own after the others: the call site - an ABI call with a 6 KB frame - then does not sit
@@ -291,20 +282,16 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
             if (!COOP || w < n) {
             const u32 li = w & bt_mask;
             const u32 inst = (tile << bt_log2) + li;
-            const bool first = w == threadIdx.x;
             u32 g0 = lb + (w >> bt_log2), g1 = g0 + 1u;   // !FUSED: work item k is tape word k
-            if (FUSED) {
-                g0 = first ? pre_g0 : __ldg(&tp.items[lb + (w >> bt_log2)]);
-                g1 = first ? pre_g1 : __ldg(&tp.items[lb + (w >> bt_log2) + 1]);
-            }
+            uint4 nxt;
+            if (FUSED) {   // three independent loads: one round trip
+                g0 = __ldg(&tp.items[lb + (w >> bt_log2)]);
+                g1 = __ldg(&tp.items[lb + (w >> bt_log2) + 1]);
+                nxt = __ldg(&tp.heads[lb + (w >> bt_log2)]);
+            } else nxt = __ldg(&tp.ops[g0]);
             // a fused work item: its words run back to back in this thread, single-use values stay in two
             // accumulator registers instead of travelling through the value store
             u32 acc0[8], acc1[8];
-            uint4 nxt = pre;
-            if (!first) {
-                if (FUSED) nxt = __ldg(&tp.heads[lb + (w >> bt_log2)]);
-                else nxt = __ldg(&tp.ops[g0]);
-            }
             for (u32 k = g0; k < g1; ++k) {
             const uint4 opw = nxt;
             bool has_value = true;   // false: the word stored its results itself / has none (asserts)
@@ -432,13 +419,6 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 if (e && inst < batch) err[inst] = 1;
                 store_slot(r, base, opw.x >> 8, bt_log2, li);
             }
-        }
-        if (threadIdx.x < ((le_next - le) << bt_log2)) {
-            if (FUSED) {   // three independent loads: one round trip
-                pre_g0 = __ldg(&tp.items[le + (threadIdx.x >> bt_log2)]);
-                pre_g1 = __ldg(&tp.items[le + (threadIdx.x >> bt_log2) + 1]);
-                pre = __ldg(&tp.heads[le + (threadIdx.x >> bt_log2)]);
-            } else pre = __ldg(&tp.ops[le + (threadIdx.x >> bt_log2)]);
         }
         lb = le;
         le = le_next;
