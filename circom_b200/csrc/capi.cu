@@ -296,10 +296,13 @@ static int get_dev_tape(const cw_circuit *c, int device, DevTape &out) {
 // builds of the interpreter: function calls (runtime tile size); fused work items (CW_FLAG_FUSE; runtime tile size, or
 // a warp per op); one operator per work item, per bit-plane mode: one instance per tile / a warp per op (tile sizes
 // fixed at compile time) / tile size as an argument
+// (the fused builds keep their accumulators in dynamic shared memory: kernels.cuh TAPE_ACC_SMEM)
 template <int PR, bool CALLS, bool BP, int BT, bool FU>
 static void launch_tape_k(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th) {
-    tape_exec_kernel<PR, CALLS, BP, BT, FU><<<tiles, th, 0, b->stream>>>(tp, b->slots, b->plane, b->bt_log2, b->first_assert_d,
-                                                                         b->err_d, b->batch);
+    constexpr u32 smem = FU ? TAPE_ACC_SMEM : 0u;
+    static_assert(TAPE_ACC_SMEM * CW_TAPE_LB <= 48u * 1024u, "the widest CTA stays within the default dynamic shared memory");
+    tape_exec_kernel<PR, CALLS, BP, BT, FU><<<tiles, th, smem * th, b->stream>>>(tp, b->slots, b->plane, b->bt_log2,
+                                                                                b->first_assert_d, b->err_d, b->batch);
 }
 template <int PR>
 static void launch_tape(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th, bool calls, bool bp, bool fused) {

@@ -245,12 +245,16 @@ __device__ __noinline__ void exec_call(const TapeDev &tp, u32 call_off, uint4 *b
 #define CW_TAPE_LB 512  // widest CTA of the interpreter (cw_batch_create clamps to it); with MINB it bounds the registers
 #endif
 #ifndef CW_TAPE_MINB
-#define CW_TAPE_MINB 2  // 512 x 2: a 64-register budget (the fused build spills ~100 bytes; measured faster than 84 registers)
+#define CW_TAPE_MINB 2  // 512 x 2: a 64-register budget (the warp-per-op builds do not spill; measured faster than 84 registers)
 #endif
 // BT >= 0 fixes the tile size at compile time (BT = 0, one instance per CTA: the slot address arithmetic then
 // folds to `base + slot * 32`; BT = 5, a warp per op); BT < 0 takes it from the launch argument.
 // FUSED: the tape has multi-word work items (CW_FLAG_FUSE); otherwise work item k IS tape word k and the item table,
 // the accumulators and the inner loop disappear at compile time.
+// The two accumulators of the fused builds live in dynamic shared memory, [accumulator][limb][threadIdx.x] (each lane
+// touches its own column: no bank conflicts, no warp barrier): in registers, their 16 words stayed live through every
+// word of an item, the Montgomery product included, and the build spilled (DESIGN §7).
+constexpr u32 TAPE_ACC_SMEM = 2 * 8 * 4;   // dynamic shared memory bytes per thread of a fused build
 template <int PRIME, bool HAS_CALLS, bool BP, int BT, bool FUSED>
 __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
     tape_exec_kernel(TapeDev tp, uint4 *__restrict__ slots, u32 *__restrict__ plane, u32 bt_log2_arg,
@@ -262,6 +266,8 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
     const u32 bt_mask = (1u << bt_log2) - 1;
     uint4 *base = slots + (((size_t)tile * tp.n_slots) << (bt_log2 + 1));
     u32 *plane_base = BP ? plane + (((size_t)tile * tp.n_bitwords) << bt_log2) : nullptr;
+    extern __shared__ uint4 tape_smem[];
+    u32 *const acc = reinterpret_cast<u32 *>(tape_smem) + threadIdx.x;   // limb i of accumulator k: acc[(8 * k + i) * blockDim.x]
     u32 lb = tp.level_start[0];
     u32 le = tp.n_levels ? tp.level_start[1] : lb;
     // (A thread's first item of a level is fetched like the others, not before the barrier: held in registers, its head
@@ -290,8 +296,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 nxt = __ldg(&tp.heads[lb + (w >> bt_log2)]);
             } else nxt = __ldg(&tp.ops[g0]);
             // a fused work item: its words run back to back in this thread, single-use values stay in two
-            // accumulator registers instead of travelling through the value store
-            u32 acc0[8], acc1[8];
+            // accumulators (shared memory) instead of travelling through the value store
             for (u32 k = g0; k < g1; ++k) {
             const uint4 opw = nxt;
             bool has_value = true;   // false: the word stored its results itself / has none (asserts)
@@ -336,11 +341,11 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 const bool half = opcode >= OP_NARROW_HALF;   // width-classed operators on operands below 2^128
                 if (FUSED && !(opw.y & OPD_CONST) && (opw.y & OPD_ACC)) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) a[i] = (opw.y & 1u) ? acc1[i] : acc0[i];
+                    for (int i = 0; i < 8; ++i) a[i] = acc[(8 * (opw.y & 1u) + i) * blockDim.x];
                 } else load_operand<BP>(a, opw.y, base, plane_base, tp.consts, bt_log2, li, half);
                 if (FUSED && !(opw.z & OPD_CONST) && (opw.z & OPD_ACC)) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) b[i] = (opw.z & 1u) ? acc1[i] : acc0[i];
+                    for (int i = 0; i < 8; ++i) b[i] = acc[(8 * (opw.z & 1u) + i) * blockDim.x];
                 } else load_operand<BP>(b, opw.z, base, plane_base, tp.consts, bt_log2, li, half);
                 if (opcode == OP_SELECT) {
                     u32 c[8];
@@ -367,10 +372,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
             if (has_value) {
                 if (FUSED && dst >= DST_ACC_DEV) {
 #pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        if (dst & 1u) acc1[i] = r[i];
-                        else acc0[i] = r[i];
-                    }
+                    for (int i = 0; i < 8; ++i) acc[(8 * (dst & 1u) + i) * blockDim.x] = r[i];
                 } else store_slot(r, base, dst, bt_log2, li);
             }
             }
