@@ -14,6 +14,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <tuple>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -182,6 +183,7 @@ struct cw_r1cs {
     std::mutex mu;
     std::map<R1csKey, DevR1cs> dev;
     cw_r1cs *eval_twin = nullptr;  // the same constraints compiled without boolean-row special cases (cw_r1cs_eval_batch)
+    cw_r1cs *qap_twin = nullptr;   // ... plus the rows a_{m+j} = w_j, j <= nPublic (cw_r1cs_quotient_*)
     bool no_bool_rows = false;
 };
 
@@ -1238,6 +1240,7 @@ int cw_r1cs_info(const cw_r1cs *r, uint64_t *n_wires, uint64_t *n_constraints, u
 void cw_r1cs_destroy(cw_r1cs *r) {
     if (!r) return;
     if (r->eval_twin) cw_r1cs_destroy(r->eval_twin);
+    if (r->qap_twin) cw_r1cs_destroy(r->qap_twin);
     for (auto &kv : r->dev) {
         cudaSetDevice(kv.first.device);
         cudaFree(kv.second.row_ptr);
@@ -1301,6 +1304,9 @@ static int get_dev_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, DevR1c
 
 struct R1csOut {
     uint4 *a = nullptr, *b = nullptr, *c = nullptr;
+    uint64_t stride = 0;     // elements between the output rows of consecutive instances
+    u32 first = 0, count = 0;   // instance window of the store
+    bool ab = false;         // c = a o b instead of C.w
 };
 
 // launches on `stream`; fb_d[batch] must hold ~0 on entry; `wide` = (n_small + 31) / 32 + 1 words of scratch for the rows the
@@ -1315,14 +1321,19 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
     rd.perm = d.perm;
     rd.n_rows = d.n_general;
     rd.prime = (u32)R.prime_id;
-    const u32 n_tiles = (S.batch + (1u << S.bt_log2) - 1) >> S.bt_log2;
+    const u32 bt_mask = (1u << S.bt_log2) - 1u;
+    const u32 n_tiles = eval ? ((eval->first + eval->count + bt_mask) >> S.bt_log2) - (eval->first >> S.bt_log2)
+                             : (S.batch + bt_mask) >> S.bt_log2;
     if (d.n_general) {
         const uint64_t items = (uint64_t)d.n_general << S.bt_log2;
         dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         // long rows: many resident warps (48 registers); short rows: the unspilled build
         const bool lean = env_int("CW_R1CS_LEAN", d.mean_row_terms >= 12 ? 1 : 0) != 0;
         EvalOut eo;
-        if (eval) { eo.a = eval->a; eo.b = eval->b; eo.c = eval->c; eo.m = R.n_constraints; }
+        if (eval) {
+            eo.a = eval->a; eo.b = eval->b; eo.c = eval->c;
+            eo.stride = eval->stride; eo.first = eval->first; eo.count = eval->count; eo.ab = eval->ab ? 1u : 0u;
+        }
 #define CW_LAUNCH_R1CS(PR)                                                                              \
     do {                                                                                                \
         if (eval) r1cs_check_kernel<PR, 3, true, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr);       \
@@ -1564,7 +1575,7 @@ int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, 
         return fail(CW_EINVAL, "bad argument");
     if (((uintptr_t)a_dev | (uintptr_t)b_dev | (uintptr_t)c_dev) & 31u) return fail(CW_EINVAL, "outputs must be 32-byte aligned");
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
-    if (b->bt_log2 != 0) return fail(CW_ESTATE, "cw_r1cs_eval_batch needs a one-instance tile layout (CW_BT_LOG2=0)");
+    if (r->data.prime_id != b->c->tape.F.prime_id) return fail(CW_EINVAL, "the R1CS and the batch use different primes");
     CU(cudaSetDevice(b->device));
     // all rows through the general path: a layout key of its own (no boolean-row special cases)
     cw_r1cs *all = nullptr;
@@ -1581,16 +1592,233 @@ int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, 
     DevR1cs d;
     int rc = get_dev_r1cs(all, b->device, b->c, d);
     if (rc) return rc;
-    StoreDev S = b->store();
-    S.slots += (size_t)first * S.n_slots * 2;
-    S.plane += (size_t)first * S.n_bitwords;
-    S.batch = count;
     R1csOut eo;
     eo.a = (uint4 *)a_dev;
     eo.b = (uint4 *)b_dev;
     eo.c = (uint4 *)c_dev;
+    eo.stride = r->data.n_constraints;
+    eo.first = first;
+    eo.count = count;
     CU(cudaMemsetAsync(b->fb_d, 0xFF, (size_t)b->batch * 8, b->stream));
-    return launch_r1cs(all, d, S, b->stream, b->fb_d, &eo, nullptr);
+    return launch_r1cs(all, d, b->store(), b->stream, b->fb_d, &eo, nullptr);
+}
+
+// ---- Groth16 quotient evaluations (the QAP step every Groth16 prover starts with) --------------------------------
+// Domain n = 2^k >= m + nPublic + 1 with k + 1 <= s (the 2-adicity of q - 1).  Values on the domain: a_i = (A.w)_i and
+// b_i = (B.w)_i for i < m, a_{m+j} = w_j for j <= nPublic, zero elsewhere; c = a o b.  Each goes to the odd coset
+// (inverse NTT, times w_2n^i, NTT) and h = a' b' - c'.
+static int qap_domain(const cw_r1cs *r, u32 &log_n, u32 &n_public) {
+    const R1csData &R = r->data;
+    const uint64_t np = (uint64_t)R.n_pub_out + R.n_pub_in;
+    if (R.n_constraints == 0) return fail(CW_EINVAL, "the R1CS has no constraints");
+    if (np + 1 > R.n_wires) return fail(CW_EINVAL, "more public signals than wires");
+    const uint64_t rows = R.n_constraints + np + 1;
+    u32 k = 0;
+    while ((1ull << k) < rows) ++k;
+    const u32 s = ntt_two_adicity(r->F);
+    if (k + 1 > s) return fail(CW_EINVAL, "the prime's 2-adicity (" + std::to_string(s) + ") admits no domain of 2^" +
+                                              std::to_string(k) + " points with its odd coset");
+    log_n = k;
+    n_public = (u32)np;
+    return CW_OK;
+}
+
+// the constraints plus the rows a_{m+j} = 1 * w_j (j <= nPublic), compiled like the eval twin (every row general)
+static cw_r1cs *qap_twin(cw_r1cs *r, u32 n_public) {
+    std::lock_guard<std::mutex> lk(r->mu);
+    if (r->qap_twin) return r->qap_twin;
+    cw_r1cs *t = new cw_r1cs();
+    t->data = r->data;
+    t->F = r->F;
+    t->no_bool_rows = true;
+    R1csData &D = t->data;
+    D.has_custom_gates = false;
+    D.gates_used.clear();
+    D.gates_applied.clear();
+    const U256 one = u256_from_u64(1);
+    u32 one_idx = (u32)D.dict.size();
+    for (size_t i = 0; i < D.dict.size(); ++i)
+        if (D.dict[i] == one) { one_idx = (u32)i; break; }
+    if (one_idx == D.dict.size()) D.dict.push_back(one);
+    for (u32 j = 0; j <= n_public; ++j) {   // row_ptr[3 m] (the end of the last row) is the start of the new row's A block
+        D.col.push_back(j);
+        D.coef.push_back(one_idx);
+        for (int k = 0; k < 3; ++k) D.row_ptr.push_back(D.col.size());
+    }
+    D.n_constraints += n_public + 1;
+    r->qap_twin = t;
+    return t;
+}
+
+// twiddle and coset-scale tables of one (device, prime, log_n), Montgomery images (ntt.cuh: ntt_tables)
+struct NttTables {
+    u32 *tw = nullptr, *shi = nullptr, *slo = nullptr;
+};
+static std::mutex g_ntt_mu;
+static std::map<std::tuple<int, int, u32>, NttTables> g_ntt_tables;   // (device, prime, log_n): kept for the process
+
+static int ntt_tables_for(int device, int prime_id, u32 log_n, NttTables &out) {
+    std::lock_guard<std::mutex> lk(g_ntt_mu);
+    auto key = std::make_tuple(device, prime_id, log_n);
+    auto it = g_ntt_tables.find(key);
+    if (it != g_ntt_tables.end()) {
+        out = it->second;
+        return CW_OK;
+    }
+    std::vector<U256> tw, shi, slo;
+    ntt_tables(make_field(prime_id), log_n, tw, shi, slo);
+    NttTables t;
+    int rc;
+    if ((rc = upload(&t.tw, tw.data(), tw.size() * 32))) return rc;
+    if ((rc = upload(&t.shi, shi.data(), shi.size() * 32))) return rc;
+    if ((rc = upload(&t.slo, slo.data(), slo.size() * 32))) return rc;
+    g_ntt_tables[key] = t;
+    out = t;
+    return CW_OK;
+}
+
+static int launch_ntt_passes(const NttPass *ps, u32 np, bool dit, const NttVecs &V, const NttTables &tb, int prime_id,
+                             cudaStream_t stream) {
+    void (*kern)(NttPass, NttVecs, const u32 *, const u32 *, const u32 *, u32) =
+        prime_id == 0 ? (dit ? ntt_pass_kernel<0, true> : ntt_pass_kernel<0, false>)
+        : prime_id == 1 ? (dit ? ntt_pass_kernel<1, true> : ntt_pass_kernel<1, false>)
+                        : (dit ? ntt_pass_kernel<-1, true> : ntt_pass_kernel<-1, false>);
+    const u32 prime = (u32)prime_id;
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 << NTT_TILE_LOG));
+    for (u32 k = 0; k < np; ++k) {
+        const NttPass &p = ps[k];
+        const u32 tiles = 1u << (p.log_n - p.b - p.log_g);
+        dim3 grid(tiles, std::min<u32>(V.n_vec, 65535u));
+        kern<<<grid, NTT_THREADS, (size_t)32 << (p.b + p.log_g), stream>>>(p, V, tb.tw, tb.shi, tb.slo, prime);
+    }
+    return CW_OK;
+}
+
+// the vectors of V (d0 + v n for v < n0, then d1) through one transform of mode NTT_MODE_*, on `stream`
+static int run_ntt(int device, int prime_id, u32 log_n, const NttVecs &V, int mode, cudaStream_t stream) {
+    NttTables tb;
+    int rc = ntt_tables_for(device, prime_id, log_n, tb);
+    if (rc) return rc;
+    NttPass dif[NTT_MAX_PASSES], dit[NTT_MAX_PASSES];
+    const u32 lg_lo = ntt_lg_lo(log_n);
+    const u32 scale = mode == NTT_MODE_FORWARD ? NTT_SCALE_NONE : mode == NTT_MODE_INVERSE ? NTT_SCALE_CONST : NTT_SCALE_COSET;
+    const u32 nd = ntt_plan(log_n, false, mode != NTT_MODE_FORWARD, scale, lg_lo, dif);
+    const u32 nt = mode == NTT_MODE_COSET ? ntt_plan(log_n, true, 0u, NTT_SCALE_NONE, lg_lo, dit) : 0u;
+    if ((rc = launch_ntt_passes(dif, nd, false, V, tb, prime_id, stream))) return rc;
+    if (mode == NTT_MODE_COSET) {
+        if ((rc = launch_ntt_passes(dit, nt, true, V, tb, prime_id, stream))) return rc;
+    } else {
+        const u32 n = 1u << log_n;
+        dim3 grid(std::max<u32>(1u, std::min<u32>((n + 255) / 256, device_sms() * 8)), std::min<u32>(V.n_vec, 65535u));
+        ntt_bitrev_kernel<<<grid, 256, 0, stream>>>(V, log_n);
+    }
+    CU(cudaGetLastError());
+    return CW_OK;
+}
+
+int cw_r1cs_qap_info(const cw_r1cs *r, uint32_t *log2_n, uint32_t *n_public) {
+    if (!r) return fail(CW_EINVAL, "null argument");
+    u32 k = 0, np = 0;
+    int rc = qap_domain(r, k, np);
+    if (rc) return rc;
+    if (log2_n) *log2_n = k;
+    if (n_public) *n_public = np;
+    return CW_OK;
+}
+
+// the domain values of the window [first, first + count) of store S, transformed and joined into h (on `stream`)
+static int quotient_on_store(cw_r1cs *r, int device, const cw_circuit *layout, const StoreDev &S, u32 first, u32 count,
+                             uint64_t *h_dev, uint64_t *scratch_dev, unsigned long long *fb_d, cudaStream_t stream) {
+    u32 k = 0, np = 0;
+    int rc = qap_domain(r, k, np);
+    if (rc) return rc;
+    cw_r1cs *t = qap_twin(r, np);
+    DevR1cs d;
+    if ((rc = get_dev_r1cs(t, device, layout, d))) return rc;
+    const uint64_t n = 1ull << k, rows = t->data.n_constraints;
+    uint4 *A = (uint4 *)h_dev, *B = (uint4 *)scratch_dev, *Cc = B + 2 * (size_t)count * n;
+    if (rows < n)
+        for (uint4 *p : {A, B, Cc}) CU(cudaMemset2DAsync(p + 2 * rows, n * 32, 0, (n - rows) * 32, count, stream));
+    R1csOut eo;
+    eo.a = A;
+    eo.b = B;
+    eo.c = Cc;
+    eo.stride = n;
+    eo.first = first;
+    eo.count = count;
+    eo.ab = true;
+    if ((rc = launch_r1cs(t, d, S, stream, fb_d, &eo, nullptr))) return rc;
+    NttVecs V;
+    V.d0 = A;
+    V.d1 = B;
+    V.n0 = count;
+    V.n_vec = 3 * count;
+    if ((rc = run_ntt(device, r->data.prime_id, k, V, NTT_MODE_COSET, stream))) return rc;
+    const size_t tot = (size_t)count * n;
+    const u32 grid = (u32)std::max<size_t>(1, std::min<size_t>((tot + 255) / 256, (size_t)device_sms() * 8));
+    if (r->data.prime_id == 0) qap_join_kernel<0><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, 0u);
+    else if (r->data.prime_id == 1) qap_join_kernel<1><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, 1u);
+    else qap_join_kernel<-1><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, (u32)r->data.prime_id);
+    CU(cudaGetLastError());
+    return CW_OK;
+}
+
+int cw_r1cs_quotient_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, uint64_t *h_dev, uint64_t *scratch_dev) {
+    if (!r || !b || !h_dev || !scratch_dev || count == 0 || (uint64_t)first + count > b->batch)
+        return fail(CW_EINVAL, "bad argument");
+    if (((uintptr_t)h_dev | (uintptr_t)scratch_dev) & 31u) return fail(CW_EINVAL, "h and scratch must be 32-byte aligned");
+    if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
+    if (r->data.prime_id != b->c->tape.F.prime_id) return fail(CW_EINVAL, "the R1CS and the batch use different primes");
+    CU(cudaSetDevice(b->device));
+    CU(cudaMemsetAsync(b->fb_d, 0xFF, (size_t)b->batch * 8, b->stream));
+    return quotient_on_store(r, b->device, b->c, b->store(), first, count, h_dev, scratch_dev, b->fb_d, b->stream);
+}
+
+int cw_r1cs_quotient_strided(cw_r1cs *r, const uint64_t *witness_dev, uint64_t stride_elems, uint32_t count, int device,
+                             uint64_t *h_dev, uint64_t *scratch_dev) {
+    if (!r || !witness_dev || !h_dev || !scratch_dev || count == 0 || stride_elems < r->data.n_wires || stride_elems >> 32)
+        return fail(CW_EINVAL, "bad argument");
+    if (((uintptr_t)witness_dev | (uintptr_t)h_dev | (uintptr_t)scratch_dev) & 31u)
+        return fail(CW_EINVAL, "device pointers must be 32-byte aligned");
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    StoreDev S;
+    S.slots = (const uint4 *)witness_dev;
+    S.plane = nullptr;
+    S.n_slots = (u32)stride_elems;
+    S.n_bitwords = 0;
+    S.bt_log2 = 0;
+    S.batch = count;
+    unsigned long long *fb_d = nullptr;
+    CU(cudaMalloc((void **)&fb_d, (size_t)count * 8));
+    rc = quotient_on_store(r, device, nullptr, S, 0, count, h_dev, scratch_dev, fb_d, 0);
+    if (!rc) {
+        cudaError_t e = cudaStreamSynchronize(0);
+        if (e != cudaSuccess) rc = fail(CW_ECUDA, cudaGetErrorString(e));
+    }
+    cudaFree(fb_d);
+    return rc;
+}
+
+int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *data_dev, int mode, int device) {
+    if (prime_id < 0 || prime_id >= CW_N_PRIMES || !data_dev || count == 0 || mode < CW_NTT_FORWARD || mode > CW_NTT_COSET)
+        return fail(CW_EINVAL, "bad argument");
+    if ((uintptr_t)data_dev & 31u) return fail(CW_EINVAL, "data must be 32-byte aligned");
+    const u32 s = ntt_two_adicity(make_field(prime_id));
+    if (log2_n < 1 || log2_n > 27 || log2_n + 1 > s)
+        return fail(CW_EINVAL, "log2_n must lie in [1, min(27, s - 1)]; the prime's 2-adicity s is " + std::to_string(s));
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    NttVecs V;
+    V.d0 = (uint4 *)data_dev;
+    V.d1 = nullptr;
+    V.n0 = count;
+    V.n_vec = count;
+    static_assert(CW_NTT_FORWARD == NTT_MODE_FORWARD && CW_NTT_INVERSE == NTT_MODE_INVERSE && CW_NTT_COSET == NTT_MODE_COSET,
+                  "transform modes");
+    if ((rc = run_ntt(device, prime_id, log2_n, V, mode, 0))) return rc;
+    CU(cudaStreamSynchronize(0));
+    return CW_OK;
 }
 
 // readWitness side of the file boundary: the 32-byte entries of a .wtns (written by this library, the reference

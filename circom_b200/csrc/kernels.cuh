@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include "fr_device.cuh"
+#include "ntt.cuh"
 #include "r1cs_small.h"
 
 namespace cw {
@@ -719,10 +720,14 @@ __device__ __forceinline__ bool r1cs_row_holds(const u32 *a, const u32 *b, const
 // MINB = CTAs per SM the register budget is cut for (r01 measurements on the bench circuit, long rows, bound by
 // memory latency: 3 -> 16.4 ms, 4 -> 13.7 ms, 5 -> 13.0 ms, 6 -> 17.0 ms per 1024 instances; circuits of short
 // rows prefer the unspilled build); the host picks by the mean row length.
-// EVAL: also leave A.w, B.w, C.w of every row in device memory ([instance][row] 32-byte elements) for a prover
+// EVAL: also leave A.w, B.w, C.w of every row in device memory for a prover, for the instances [first, first + count)
+// of the store (any tile layout): row `row` of instance first + i at element i * stride + row.  ab: write a o b instead of
+// C.w (the pointwise product a Groth16 prover uses; the C terms are not read).
 struct EvalOut {
     uint4 *a = nullptr, *b = nullptr, *c = nullptr;
-    unsigned long long m = 0;  // rows per instance
+    unsigned long long stride = 0;  // elements between the rows of consecutive instances
+    u32 first = 0, count = 0;
+    u32 ab = 0;
 };
 // FILTER: the rows of R.perm are the integer rows (r1cs_small_kernel below); only those it marked in `filter` are decided
 template <int PRIME, int MINB, bool EVAL, bool FILTER>
@@ -730,15 +735,18 @@ __global__ void __launch_bounds__(256, MINB) r1cs_check_kernel(R1csDev R, StoreD
                                                          EvalOut out, const u32 *__restrict__ filter) {
     const FrParams &P = CW_FR(PRIME, R.prime);
     const u32 bt_mask = (1u << S.bt_log2) - 1u;
-    const u32 n_tiles = (S.batch + bt_mask) >> S.bt_log2;
+    // (EVAL: the tiles that hold the window)
+    const u32 t_begin = EVAL ? out.first >> S.bt_log2 : 0u;
+    const u32 n_tiles = EVAL ? (out.first + out.count + bt_mask) >> S.bt_log2 : (S.batch + bt_mask) >> S.bt_log2;
     const unsigned long long n_items = (unsigned long long)R.n_rows << S.bt_log2;
-    for (u32 tile = blockIdx.y; tile < n_tiles; tile += gridDim.y) {
+    for (u32 tile = t_begin + blockIdx.y; tile < n_tiles; tile += gridDim.y) {
         const uint4 *tb = store_tile(S, tile);
         const u32 *pb = store_plane(S, tile);
         for (unsigned long long w = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; w < n_items;
              w += (unsigned long long)gridDim.x * blockDim.x) {
             const u32 li = (u32)w & bt_mask, inst = (tile << S.bt_log2) + li;
             if (inst >= S.batch) continue;
+            if (EVAL && (inst < out.first || inst - out.first >= out.count)) continue;
             if (FILTER) {
                 if (!filter[(R.n_rows + 31u) >> 5]) return;   // the word after the bitmap: no row was marked at all
                 const u32 k = (u32)(w >> S.bt_log2);
@@ -750,9 +758,13 @@ __global__ void __launch_bounds__(256, MINB) r1cs_check_kernel(R1csDev R, StoreD
             u32 a[8], b[8], c[8];
             r1cs_lc<PRIME>(a, R, p0, p1, S, tb, pb, li, P, &first_bad[inst]);
             r1cs_lc<PRIME>(b, R, p1, p2, S, tb, pb, li, P, &first_bad[inst]);
-            r1cs_lc<PRIME>(c, R, p2, p3, S, tb, pb, li, P, &first_bad[inst]);
+            if (EVAL && out.ab) {
+                u32 am[8];
+                fr_to_mont(am, a, P);
+                fr_mont_mul(c, am, b, P);
+            } else r1cs_lc<PRIME>(c, R, p2, p3, S, tb, pb, li, P, &first_bad[inst]);
             if (EVAL) {
-                const size_t o = ((size_t)inst * out.m + row) * 2;
+                const size_t o = ((size_t)(inst - out.first) * out.stride + row) * 2;
                 stg256(out.a + o, a);
                 stg256(out.b + o, b);
                 stg256(out.c + o, c);
@@ -910,6 +922,82 @@ __global__ void fr_mul_bench_kernel(uint4 *__restrict__ data, size_t n, int iter
     }
     data[2 * i] = make_uint4(x[0], x[1], x[2], x[3]);
     data[2 * i + 1] = make_uint4(x[4], x[5], x[6], x[7]);
+}
+
+// ---- batched NTT (ntt.cuh) ----------------------------------------------------------------------------------------
+// One pass of `count` transforms: blockIdx.x = tile of a vector, blockIdx.y walks the vectors (vector v lives at d0 + v n
+// for v < n0, else at d1 + (v - n0) n).  The tile moves global -> shared once, runs p.b stages there, and moves back.
+// 64 KB of shared memory and 256 threads per CTA: three CTAs per SM.
+struct NttVecs {
+    uint4 *d0, *d1;
+    u32 n0, n_vec;
+};
+__device__ __forceinline__ uint4 *ntt_vec(const NttVecs &V, u32 v, u32 log_n) {
+    return v < V.n0 ? V.d0 + ((size_t)v << (log_n + 1)) : V.d1 + ((size_t)(v - V.n0) << (log_n + 1));
+}
+template <int PRIME, bool DIT>
+__global__ void __launch_bounds__(NTT_THREADS, 3) ntt_pass_kernel(NttPass p, NttVecs V, const u32 *__restrict__ tw,
+                                                                 const u32 *__restrict__ shi, const u32 *__restrict__ slo,
+                                                                 u32 prime) {
+    extern __shared__ u32 ntt_sm[];
+    const FrParams &P = CW_FR(PRIME, prime);
+    const u32 T = 1u << (p.b + p.log_g);
+    for (u32 v = blockIdx.y; v < V.n_vec; v += gridDim.y) {
+        uint4 *x = ntt_vec(V, v, p.log_n);
+        for (u32 e = threadIdx.x; e < T; e += NTT_THREADS) {
+            const size_t i = ntt_gidx(p, blockIdx.x, e);
+            const uint4 lo = x[2 * i], hi = x[2 * i + 1];
+            ntt_sm[0 * T + e] = lo.x; ntt_sm[1 * T + e] = lo.y; ntt_sm[2 * T + e] = lo.z; ntt_sm[3 * T + e] = lo.w;
+            ntt_sm[4 * T + e] = hi.x; ntt_sm[5 * T + e] = hi.y; ntt_sm[6 * T + e] = hi.z; ntt_sm[7 * T + e] = hi.w;
+        }
+        __syncthreads();
+        for (u32 tt = 0; tt < p.b; ++tt) {
+            const u32 t = DIT ? tt : p.b - 1u - tt;
+            for (u32 q = threadIdx.x; q < T / 2u; q += NTT_THREADS) ntt_butterfly(ntt_sm, T, p, blockIdx.x, t, q, tw, DIT, P);
+            __syncthreads();
+        }
+        for (u32 e = threadIdx.x; e < T; e += NTT_THREADS) {
+            const u32 i = ntt_gidx(p, blockIdx.x, e);
+            u32 r[8];
+#pragma unroll
+            for (int l = 0; l < 8; ++l) r[l] = ntt_sm[l * T + e];
+            if (p.scale != NTT_SCALE_NONE) ntt_scale(r, i, p, shi, slo, P);
+            x[2 * (size_t)i] = make_uint4(r[0], r[1], r[2], r[3]);
+            x[2 * (size_t)i + 1] = make_uint4(r[4], r[5], r[6], r[7]);
+        }
+        __syncthreads();
+    }
+}
+
+// natural <-> bit-reversed order in place (each pair swapped by its lower index)
+__global__ void __launch_bounds__(256) ntt_bitrev_kernel(NttVecs V, u32 log_n) {
+    const u32 n = 1u << log_n;
+    for (u32 v = blockIdx.y; v < V.n_vec; v += gridDim.y) {
+        uint4 *x = ntt_vec(V, v, log_n);
+        for (u32 i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+            const u32 r = ntt_bitrev(i, log_n);
+            if (i < r) {
+                const uint4 a0 = x[2 * (size_t)i], a1 = x[2 * (size_t)i + 1], b0 = x[2 * (size_t)r], b1 = x[2 * (size_t)r + 1];
+                x[2 * (size_t)i] = b0; x[2 * (size_t)i + 1] = b1;
+                x[2 * (size_t)r] = a0; x[2 * (size_t)r + 1] = a1;
+            }
+        }
+    }
+}
+
+// h = a * b - c elementwise over `n` elements (h may alias a)
+template <int PRIME>
+__global__ void __launch_bounds__(256) qap_join_kernel(uint4 *h, const uint4 *a, const uint4 *__restrict__ b,
+                                                       const uint4 *__restrict__ c, size_t n, u32 prime) {
+    const FrParams &P = CW_FR(PRIME, prime);
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        u32 x[8], y[8], z[8], r[8];
+        ldg256(x, a + 2 * i);
+        ldg256_nc(y, b + 2 * i);
+        ldg256_nc(z, c + 2 * i);
+        qap_join(r, x, y, z, P);
+        stg256(h + 2 * i, r);
+    }
 }
 
 #endif  // CW_KERNELS_TAPE_ONLY

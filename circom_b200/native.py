@@ -16,6 +16,7 @@ CW_FLAG_NO_ASSERTS, CW_FLAG_HOST_ONLY, CW_FLAG_O0, CW_FLAG_NO_PEEPHOLE, CW_FLAG_
 CW_FLAG_COMPACT = CW_FLAG_BITPLANE | CW_FLAG_REUSE
 CW_FLAG_FUSE = 64
 CW_FLAG_NO_NARROW = 128
+CW_NTT_FORWARD, CW_NTT_INVERSE, CW_NTT_COSET = 0, 1, 2
 
 
 class CwError(RuntimeError):
@@ -85,6 +86,10 @@ def _load() -> ctypes.CDLL:
         "cw_batch_expand_witness": (c_int, [P, c_uint32, c_uint32, c_void_p]),
         "cw_r1cs_check_batch": (c_int, [P, P, c_void_p, POINTER(c_float)]),
         "cw_r1cs_eval_batch": (c_int, [P, P, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_r1cs_qap_info": (c_int, [P, POINTER(c_uint32), POINTER(c_uint32)]),
+        "cw_r1cs_quotient_batch": (c_int, [P, P, c_uint32, c_uint32, c_void_p, c_void_p]),
+        "cw_r1cs_quotient_strided": (c_int, [P, c_void_p, c_uint64, c_uint32, c_int, c_void_p, c_void_p]),
+        "cw_fr_ntt_batch": (c_int, [c_int, c_uint32, c_uint32, c_void_p, c_int, c_int]),
         "cw_comm_unique_id": (c_int, [c_void_p]),
         "cw_comm_init": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),
         "cw_comm_from_nccl": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),

@@ -459,6 +459,23 @@ class R1cs:
         check(lib.cw_r1cs_eval_batch(self._h, b._h, first, count, ctypes.c_void_p(a_ptr), ctypes.c_void_p(b_ptr),
                                      ctypes.c_void_p(c_ptr)))
 
+    def qap_info(self):
+        """(log2 n, nPublic): the Groth16 evaluation domain of this constraint system (include/circom_b200.h)"""
+        k, npub = ctypes.c_uint32(), ctypes.c_uint32()
+        check(lib.cw_r1cs_qap_info(self._h, ctypes.byref(k), ctypes.byref(npub)))
+        return k.value, npub.value
+
+    def quotient_batch(self, b: "Batch", first: int, count: int, h_ptr: int, scratch_ptr: int) -> None:
+        """h = a'b' - c' of instances [first, first+count) into device array [count][n][4] uint64; scratch: 2*count*n*32
+        bytes of device memory.  Asynchronous on the batch stream (b.sync())."""
+        check(lib.cw_r1cs_quotient_batch(self._h, b._h, first, count, ctypes.c_void_p(h_ptr), ctypes.c_void_p(scratch_ptr)))
+
+    def quotient(self, device_ptr: int, count: int, stride: Optional[int], h_ptr: int, scratch_ptr: int,
+                 device: int = 0) -> None:
+        """the same for `count` dense witness rows on the device, `stride` 32-byte elements apart (None: n_wires)"""
+        check(lib.cw_r1cs_quotient_strided(self._h, ctypes.c_void_p(device_ptr), stride or self.n_wires, count, device,
+                                           ctypes.c_void_p(h_ptr), ctypes.c_void_p(scratch_ptr)))
+
     def write(self, path: str, n_pub_out: Optional[int] = None, n_pub_in: Optional[int] = None,
               n_prv_in: Optional[int] = None) -> None:
         """None keeps the count the circuit / the loaded file carries (the header feeds snarkjs' public-signal count)"""
@@ -482,6 +499,11 @@ class R1cs:
         fb = np.zeros(batch, dtype=np.int64)
         check(lib.cw_r1cs_check(self._h, w.ctypes.data, 0, batch, device, fb.ctypes.data, ctypes.byref(ms)))
         return fb, ms.value
+
+
+def ntt_batch(prime_id: int, log2_n: int, count: int, data_ptr: int, mode: int, device: int = 0) -> None:
+    """in-place transforms of `count` device vectors [count][2^log2_n][4] uint64 (mode: CW_NTT_FORWARD / INVERSE / COSET)"""
+    check(lib.cw_fr_ntt_batch(prime_id, log2_n, count, ctypes.c_void_p(data_ptr), mode, device))
 
 
 class WitnessCalculator:

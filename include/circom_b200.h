@@ -263,9 +263,37 @@ int cw_r1cs_check_batch(cw_r1cs *r, cw_batch *b, int64_t *first_bad, float *kern
 int cw_r1cs_compiled_info(cw_r1cs *r, cw_batch *b, int device, uint64_t info[4]);
 /* A.w, B.w, C.w of every constraint for instances [first, first + count) of a batch, left in device memory
  * ([count][n_constraints][4] uint64 each, canonical, 32-byte aligned) for the prover stage that follows witness
- * generation; asynchronous on the batch stream (cw_batch_sync).  One-instance tile layouts only. */
+ * generation; asynchronous on the batch stream (cw_batch_sync).  Any tile layout, any first. */
 int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, uint64_t *a_dev, uint64_t *b_dev,
                        uint64_t *c_dev);
+
+/* ---- Groth16 quotient evaluations: what a prover's H multi-exponentiation consumes ---------------------------------
+ * The convention of the snarkjs Groth16 prover (buildABC1 -> ifft -> shift -> fft -> joinABC) and of rapidsnark up to
+ * its H multiexp, written out here (byte compatibility with those tools' buffers is not verified by this library):
+ *   s = 2-adicity of q - 1, g = smallest quadratic non-residue counted up from 2, w_{2^j} = g^((q-1)/2^s * 2^(s-j)).
+ *   m = constraints, nPublic = n_pub_out + n_pub_in of the R1CS (from a circuit: its outputs), w = witness.
+ *   n = 2^k, the smallest power of two >= m + nPublic + 1, with k + 1 <= s (else CW_EINVAL; grumpkin and secq256r1 have
+ *   s = 1).  a_i = (A.w)_i, b_i = (B.w)_i for i < m; a_{m+j} = w_j for j <= nPublic (w_0 = 1); zero elsewhere;
+ *   c = a o b (pointwise; C.w is not used).  X' = X-hat(w_2n w_n^j) with X-hat the inverse NTT of X.
+ *   h_j = a'_j b'_j - c'_j, j < n, natural order, canonical 4 x u64 limbs. */
+int cw_r1cs_qap_info(const cw_r1cs *r, uint32_t *log2_n, uint32_t *n_public);   /* host only */
+/* h of instances [first, first + count) of a batch that has run, read where the tape left the witnesses (any tile
+ * layout and value store).  h_dev: [count][n][4] u64; scratch_dev: 2 * count * n * 32 bytes; both device memory, 32-byte
+ * aligned, owned by the caller.  Asynchronous on the batch stream (cw_batch_sync). */
+int cw_r1cs_quotient_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, uint64_t *h_dev, uint64_t *scratch_dev);
+/* the same for dense witness rows on `device` (row i at witness_dev + i * stride_elems * 4, as cw_r1cs_check_strided
+ * reads them: e.g. .wtns files read with cw_wtns_read and copied up).  Runs on the legacy default stream and returns
+ * when h is complete. */
+int cw_r1cs_quotient_strided(cw_r1cs *r, const uint64_t *witness_dev, uint64_t stride_elems, uint32_t count, int device,
+                             uint64_t *h_dev, uint64_t *scratch_dev);
+/* `count` in-place transforms of [count][2^log2_n][4] u64 canonical vectors in natural order, 1 <= log2_n <= 27 and
+ * log2_n + 1 <= s (CW_EINVAL otherwise).  FORWARD: X_j = sum_i x_i w_n^(ij); INVERSE: x_i = 1/n sum_j X_j w_n^(-ij);
+ * COSET: X'_j = sum_i xh_i w_2n^i w_n^(ij) with xh = INVERSE(X) - the transform the quotient applies to each
+ * polynomial.  Runs on the legacy default stream and returns when done (the parity surface of the transform). */
+#define CW_NTT_FORWARD 0
+#define CW_NTT_INVERSE 1
+#define CW_NTT_COSET 2
+int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *data_dev, int mode, int device);
 
 /* ---- multi-GPU: one process per GPU, independent inputs sharded over the ranks ---------------------------
  * The reference has no distributed mode (Circom_CalcWit is per-process state, calcwit.cpp:26-45).  Here rank 0
