@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <bitset>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <stdexcept>
@@ -1495,7 +1496,12 @@ struct Lowerer {
         // post order with at most two live accumulators (deeper sub-tree first; a second fused operand may only be a
         // chain), at most FUSE_MAX operators per work item.  The DAG gets shallower (levels are recomputed over the
         // groups) and narrower in memory traffic; each group still writes exactly one value (its root's).
+        // A bit field (BITS) is fused too: runs of bits are only formed from work items of one word, so a fused BITS
+        // is always a single field, which the interpreter evaluates like any other operator.
         constexpr uint32_t FUSE_MAX = 24;
+        // why single-reader values that are not witness entries stay in the value store (CW_FUSION_CENSUS=1 prints it)
+        enum { FR_READER, FR_POSITION, FR_SIZE, FR_CHAIN, FR_N };
+        uint64_t refused[FR_N] = {}, refused_op[64] = {};
         std::vector<uint8_t> fusedf(n_prov, 0);          // op is evaluated inside its reader's work item
         std::vector<uint32_t> kid_a(n_prov, NO_SLOT), kid_b(n_prov, NO_SLOT);  // fused producers of operands a / b (op index)
         {
@@ -1531,14 +1537,12 @@ struct Lowerer {
                 const size_t c = slot - n_pre;
                 const uint32_t opc = pops[c * 4];
                 if (uses[slot] != 1 || cons[slot] != reader || cons_pos[slot] != pos || claimed[slot] >= 0) return false;
-                if (is_assert_op(opc) || opc == 45 || opc == 47 || opc == DOP_BITS || opc == CW_OP_COPY) return false;
+                if (is_assert_op(opc) || opc == 45 || opc == 47 || opc == CW_OP_COPY) return false;
                 if (opc == CW_OP_INV || opc == CW_OP_POW) return false;   // (run in a pass of their own: items of one word)
                 return true;
             };
-            for (size_t i = 0; i < n_prov; ++i) {
-                if (!live[n_pre + i]) continue;
+            auto decide = [&](size_t i) {
                 const uint32_t *o = &pops[i * 4];
-                if (o[0] == 45 || o[0] == 47 || o[0] == CW_OP_INV || o[0] == CW_OP_POW) continue;
                 uint32_t ka = candidate(o[1], i, 1) ? o[1] - n_pre : NO_SLOT;
                 uint32_t kb = candidate(o[2], i, 2) ? o[2] - n_pre : NO_SLOT;
                 if (ka != NO_SLOT && kb != NO_SLOT) {
@@ -1548,11 +1552,12 @@ struct Lowerer {
                         // keep the larger tree, give the other its own work item
                         uint32_t drop = gsize[ka] >= gsize[kb] ? kb : ka;
                         if (need[other] > 1) drop = other;
+                        ++refused[need[other] > 1 ? FR_CHAIN : FR_SIZE];
                         if (drop == ka) ka = NO_SLOT; else kb = NO_SLOT;
                     }
                 }
-                if (ka != NO_SLOT && kb == NO_SLOT && gsize[ka] + 1 > FUSE_MAX) ka = NO_SLOT;
-                if (kb != NO_SLOT && ka == NO_SLOT && gsize[kb] + 1 > FUSE_MAX) kb = NO_SLOT;
+                if (ka != NO_SLOT && kb == NO_SLOT && gsize[ka] + 1 > FUSE_MAX) { ka = NO_SLOT; ++refused[FR_SIZE]; }
+                if (kb != NO_SLOT && ka == NO_SLOT && gsize[kb] + 1 > FUSE_MAX) { kb = NO_SLOT; ++refused[FR_SIZE]; }
                 kid_a[i] = ka;
                 kid_b[i] = kb;
                 uint32_t sz = 1;
@@ -1566,6 +1571,63 @@ struct Lowerer {
                 need[i] = nd;
                 if (ka != NO_SLOT) fusedf[ka] = 1;
                 if (kb != NO_SLOT) fusedf[kb] = 1;
+            };
+            // A sum of two fused sums that both need two accumulators, i = q + p with p = u + v the later of the two, is
+            // regrouped as i = p' + v with p' = q + u: then no subtree needs a third accumulator.  Field addition is
+            // associative, and p has no reader but i and is no witness entry, so only p's own value changes; its static
+            // width is recomputed (the width classes of p' and i are chosen from it when the tape words are written).
+            auto opd_width = [&](uint32_t x) -> uint32_t {
+                if (x & OPERAND_CONST) return (uint32_t)u256_bitlen(consts[x & 0x7FFFFFFFu]);
+                return slot_bits[x];
+            };
+            auto regroup = [&](size_t i) {
+                uint32_t *o = &pops[i * 4];
+                if (o[0] != CW_OP_ADD || !candidate(o[1], i, 1) || !candidate(o[2], i, 2)) return;
+                const uint32_t a = o[1] - n_pre, b = o[2] - n_pre, p = std::max(a, b), q = std::min(a, b);
+                uint32_t *op = &pops[(size_t)p * 4];
+                if (need[q] < 2 || need[p] < 2 || op[0] != CW_OP_ADD || gsize[p] + gsize[q] + 1 > FUSE_MAX) return;
+                if ((kid_a[p] != NO_SLOT && need[kid_a[p]] > 1) || (kid_b[p] != NO_SLOT && need[kid_b[p]] > 1)) return;
+                const uint32_t u = op[1], v = op[2];
+                if (kid_a[p] != NO_SLOT) fusedf[kid_a[p]] = 0;
+                if (kid_b[p] != NO_SLOT) fusedf[kid_b[p]] = 0;
+                op[1] = n_pre + q;
+                op[2] = u;
+                o[1] = n_pre + p;
+                o[2] = v;
+                cons[n_pre + q] = (uint32_t)p;
+                cons_pos[n_pre + q] = 1;
+                cons_pos[n_pre + p] = 1;
+                if (!(u & OPERAND_CONST) && uses[u] == 1) { cons[u] = p; cons_pos[u] = 2; }
+                if (!(v & OPERAND_CONST) && uses[v] == 1) { cons[v] = (uint32_t)i; cons_pos[v] = 2; }
+                const uint32_t w = std::max(opd_width(n_pre + q), opd_width(u)) + 1;
+                slot_bits[n_pre + p] = (uint16_t)(w <= qb() - 1 ? w : 256u);
+                decide(p);
+            };
+            for (size_t i = 0; i < n_prov; ++i) {
+                if (!live[n_pre + i]) continue;
+                const uint32_t opc = pops[i * 4];
+                if (opc == 45 || opc == 47 || opc == CW_OP_INV || opc == CW_OP_POW) continue;
+                regroup(i);
+                decide(i);
+            }
+            const char *cenv = getenv("CW_FUSION_CENSUS");
+            if (fuse_on && cenv && atoi(cenv)) {
+                // the values the loop above never offered (those it dropped are counted there)
+                for (size_t c = 0; c < n_prov; ++c) {
+                    const uint32_t s = n_pre + (uint32_t)c, opc = pops[c * 4];
+                    if (!live[s] || fusedf[c] || uses[s] != 1 || claimed[s] >= 0 || is_assert_op(opc)) continue;
+                    const uint32_t rd = pops[(size_t)cons[s] * 4];
+                    if (rd == 45 || rd == 47 || rd == CW_OP_INV || rd == CW_OP_POW) ++refused[FR_READER];
+                    else if (cons_pos[s] == 3) ++refused[FR_POSITION];
+                    else if (!candidate(s, cons[s], cons_pos[s])) ++refused_op[opc & 63u];
+                }
+                fprintf(stderr, "fusion census: single-reader values kept in the store: reader INV/POW %llu, operand c %llu, "
+                        "FUSE_MAX %llu, chain rule %llu, producer opcode",
+                        (unsigned long long)refused[FR_READER], (unsigned long long)refused[FR_POSITION],
+                        (unsigned long long)refused[FR_SIZE], (unsigned long long)refused[FR_CHAIN]);
+                for (int k = 0; k < 64; ++k)
+                    if (refused_op[k]) fprintf(stderr, " %d:%llu", k, (unsigned long long)refused_op[k]);
+                fprintf(stderr, "\n");
             }
         }
         // levels over the groups (a group reads the external operands of all its operators, writes its root's value)
