@@ -23,7 +23,10 @@
 #include <vector>
 
 #include "../../include/circom_b200.h"
+#include <cub/device/device_radix_sort.cuh>
+
 #include "kernels.cuh"
+#include "msm.cuh"
 #include "tape_calls.h"
 #include "tape.h"
 #include "hostpack.h"
@@ -1818,6 +1821,185 @@ int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *dat
                   "transform modes");
     if ((rc = run_ntt(device, prime_id, log2_n, V, mode, 0))) return rc;
     CU(cudaStreamSynchronize(0));
+    return CW_OK;
+}
+
+// ---- multi-scalar multiplication on G1 of BN254 (msm.cuh) -------------------------------------------------------------
+struct cw_g1_bases {
+    int device = 0;
+    uint64_t n = 0;
+    u32 *pts = nullptr;   // [n][16] u32: Montgomery x, y; (0, 0) = infinity
+};
+
+static const uint64_t MSM_MAX_N = 1ull << 26;
+static const size_t MSM_CHUNK_BYTES = (size_t)2 << 30;   // scratch of one chunk of instances, about
+
+// the scratch of one chunk of `chunk` instances: offsets into the caller's buffer (each 256-byte aligned)
+struct MsmPlan {
+    u32 c = 0, W = 0, B = 0, chunk = 0;
+    uint64_t n = 0, items = 0, slots[2] = {0, 0};
+    size_t keys[2], vals[2], cub, cub_bytes = 0, buckets, lv_keys[2], lv_pts[2], segs, wins, total = 0;
+};
+static u32 msm_seg_bits(u32 segs) {   // bits of the largest segment index
+    u32 b = 0;
+    while (b < 32 && ((uint64_t)1 << b) < segs) ++b;
+    return b;
+}
+static int msm_plan(uint64_t n, u32 chunk, MsmPlan &p) {
+    p.n = n;
+    const int cw = env_int("CW_MSM_WINDOW", 0);   // (window sweeps: scripts/msm_bench.py)
+    p.c = cw >= (int)MSM_MIN_C && cw <= (int)MSM_MAX_C ? (u32)cw : msm_window_bits(n);
+    p.W = msm_windows(p.c);
+    p.B = 1u << (p.c - 1);
+    p.chunk = chunk;
+    p.items = (uint64_t)chunk * p.W * n;
+    p.slots[0] = msm_level_out(p.items);
+    p.slots[1] = msm_level_out(p.slots[0]);
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, p.cub_bytes, (const u32 *)nullptr, (u32 *)nullptr, (const u32 *)nullptr,
+                                       (u32 *)nullptr, (int)p.items, 0, (int)(p.c + msm_seg_bits(chunk * p.W))));
+    size_t at = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = at;
+        at += (bytes + 255) & ~(size_t)255;
+        return o;
+    };
+    for (int k = 0; k < 2; ++k) {
+        p.keys[k] = take(p.items * 4);
+        p.vals[k] = take(p.items * 4);
+    }
+    p.cub = take(p.cub_bytes);
+    p.buckets = take((size_t)chunk * p.W * p.B * sizeof(Xyzz));
+    for (int k = 0; k < 2; ++k) {
+        p.lv_keys[k] = take(p.slots[k] * 4);
+        p.lv_pts[k] = take(p.slots[k] * sizeof(Xyzz));
+    }
+    const u32 m = p.B < MSM_SEG ? p.B : MSM_SEG;
+    p.segs = take((size_t)chunk * p.W * (p.B / m) * sizeof(Xyzz));
+    p.wins = take((size_t)chunk * p.W * sizeof(Xyzz));
+    p.total = at;
+    return CW_OK;
+}
+// the chunk size for `count` instances of n points: bounded by MSM_CHUNK_BYTES, the 32-bit keys and int item counts
+static int msm_plan_for(uint64_t n, u32 count, MsmPlan &p) {
+    MsmPlan one;
+    int rc = msm_plan(n, 1, one);
+    if (rc) return rc;
+    uint64_t chunk = std::max<uint64_t>(1, MSM_CHUNK_BYTES / one.total);
+    chunk = std::min<uint64_t>(chunk, count);
+    chunk = std::min<uint64_t>(chunk, ((1ull << (32 - one.c)) - 1) / one.W);
+    chunk = std::min<uint64_t>(chunk, std::max<uint64_t>(1, (uint64_t)INT32_MAX / (one.W * n)));
+    return msm_plan(n, (u32)chunk, p);
+}
+
+int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g1_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G1 bases are built for bn128 (BN254) only");
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    const FieldParams F = make_field(MSM_PRIME);
+    const U256 three = F.to_mont(u256_from_u64(3));
+    std::vector<U256> mont(2 * n);
+    for (uint64_t i = 0; i < n; ++i) {
+        U256 x, y;
+        memcpy(x.v, points + 8 * i, 32);
+        memcpy(y.v, points + 8 * i + 4, 32);
+        if (x.is_zero() && y.is_zero()) {
+            mont[2 * i] = x;
+            mont[2 * i + 1] = y;
+            continue;
+        }
+        if (!(x < F.q) || !(y < F.q)) return fail(CW_EINVAL, "point " + std::to_string(i) + ": a coordinate is not below q");
+        const U256 xm = F.to_mont(x), ym = F.to_mont(y);
+        if (F.mont_mul(ym, ym) != F.addm(F.mont_mul(F.mont_mul(xm, xm), xm), three))
+            return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the curve y^2 = x^3 + 3");
+        mont[2 * i] = xm;
+        mont[2 * i + 1] = ym;
+    }
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    cw_g1_bases *b = new cw_g1_bases();
+    b->device = device;
+    b->n = n;
+    if ((rc = upload(&b->pts, mont.data(), (size_t)n * 64))) {
+        delete b;
+        return rc;
+    }
+    *out = b;
+    return CW_OK;
+}
+
+void cw_g1_bases_destroy(cw_g1_bases *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    cudaFree(b->pts);
+    delete b;
+}
+
+int cw_g1_msm_scratch_bytes(const cw_g1_bases *b, uint32_t count, uint64_t *bytes) {
+    if (!b || !bytes || count == 0) return fail(CW_EINVAL, "bad argument");
+    int rc = ensure_device(b->device);
+    if (rc) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p))) return rc;
+    *bytes = p.total;
+    return CW_OK;
+}
+
+int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                    uint64_t *out_dev, void *scratch_dev, void *stream) {
+    if (!b || !scalars_dev || !out_dev || !scratch_dev || count == 0) return fail(CW_EINVAL, "bad argument");
+    if (stride_elems < b->n) return fail(CW_EINVAL, "stride_elems must be at least the number of points");
+    if (((uintptr_t)scalars_dev | (uintptr_t)out_dev | (uintptr_t)scratch_dev) & 31u)
+        return fail(CW_EINVAL, "device pointers must be 32-byte aligned");
+    int rc = ensure_device(b->device);
+    if (rc) return rc;
+    for (const void *p : {(const void *)scalars_dev, (const void *)out_dev, (const void *)scratch_dev}) {
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+            cudaGetLastError();
+            return fail(CW_EINVAL, "not a device pointer");
+        }
+        if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return fail(CW_EINVAL, "not device memory");
+        if (a.device != b->device) return fail(CW_EINVAL, "device memory of another device than the bases'");
+    }
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char *S = (char *)scratch_dev;
+    const u32 n = (u32)b->n, sms = device_sms();
+    const u32 m = p.B < MSM_SEG ? p.B : MSM_SEG, per = p.B / m;
+    for (u32 i0 = 0; i0 < count; i0 += p.chunk) {
+        const u32 cn = std::min(p.chunk, count - i0), n_win = cn * p.W;
+        const uint64_t N = (uint64_t)n_win * n;
+        u32 *k0 = (u32 *)(S + p.keys[0]), *k1 = (u32 *)(S + p.keys[1]), *v0 = (u32 *)(S + p.vals[0]), *v1 = (u32 *)(S + p.vals[1]);
+        dim3 grid(std::max<u32>(1, std::min<u32>((n + MSM_THREADS - 1) / MSM_THREADS, sms * 8)), std::min<u32>(cn, 65535u));
+        msm_digits_kernel<<<grid, MSM_THREADS, 0, st>>>((const uint4 *)(scalars_dev + 4 * (size_t)i0 * stride_elems),
+                                                        stride_elems, n, p.c, p.W, cn, k0, v0);
+        size_t cub_bytes = p.cub_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(S + p.cub, cub_bytes, k0, k1, v0, v1, (int)N, 0, (int)(p.c + msm_seg_bits(n_win)), st));
+        Xyzz *buckets = (Xyzz *)(S + p.buckets);
+        CU(cudaMemsetAsync(buckets, 0, (size_t)n_win * p.B * sizeof(Xyzz), st));
+        // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
+        uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
+        int lv = 0;
+        msm_runs_kernel<true><<<(u32)((threads + MSM_THREADS - 1) / MSM_THREADS), MSM_THREADS, 0, st>>>(
+            k1, v1, b->pts, nullptr, N, p.c, buckets, (u32 *)(S + p.lv_keys[0]), (Xyzz *)(S + p.lv_pts[0]));
+        while (threads > 1) {
+            items = msm_level_out(items);
+            threads = (items + MSM_RUN - 1) / MSM_RUN;
+            msm_runs_kernel<false><<<(u32)((threads + MSM_THREADS - 1) / MSM_THREADS), MSM_THREADS, 0, st>>>(
+                (const u32 *)(S + p.lv_keys[lv]), nullptr, nullptr, (const Xyzz *)(S + p.lv_pts[lv]), items, p.c, buckets,
+                (u32 *)(S + p.lv_keys[lv ^ 1]), (Xyzz *)(S + p.lv_pts[lv ^ 1]));
+            lv ^= 1;
+        }
+        Xyzz *segs = (Xyzz *)(S + p.segs), *wins = (Xyzz *)(S + p.wins);
+        const uint64_t seg_threads = (uint64_t)n_win * per;
+        msm_segments_kernel<<<(u32)((seg_threads + MSM_THREADS - 1) / MSM_THREADS), MSM_THREADS, 0, st>>>(buckets, p.B, n_win, segs);
+        msm_windows_kernel<<<n_win, MSM_THREADS, 0, st>>>(segs, per, wins);
+        msm_final_kernel<<<(cn + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(wins, p.W, p.c, cn,
+                                                                                      (uint4 *)(out_dev + 8 * (size_t)i0));
+        CU(cudaGetLastError());
+    }
     return CW_OK;
 }
 

@@ -295,6 +295,35 @@ int cw_r1cs_quotient_strided(cw_r1cs *r, const uint64_t *witness_dev, uint64_t s
 #define CW_NTT_COSET 2
 int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *data_dev, int mode, int device);
 
+/* ---- multi-scalar multiplication on G1 -----------------------------------------------------------------------------
+ * The prover's MSMs after the quotient: H = sum_j h_j H_j over the proving key's H points, and A, B1, C = sum_i w_i P_i.
+ *   G1 of BN254 is y^2 = x^3 + 3 over the base field q (the grumpkin prime, CW_PRIME_GRUMPKIN).  Its order is r, the
+ *   bn128 prime; the cofactor is 1 and the generator is (1, 2).
+ *   A point at the ABI is affine: x then y, each 4 x u64 canonical limbs, 64 bytes per point.  The point at infinity is
+ *   (0, 0), which is not on the curve, so the encoding is unambiguous.
+ *   The result is sum_i s_i P_i with s_i taken as a 256-bit integer: any 256 bits are valid input, and s and s mod r give
+ *   the same point (no scalar is checked).
+ * snarkjs' .zkey stores points as Montgomery images; convert them to canonical form first. */
+typedef struct cw_g1_bases cw_g1_bases;
+/* n points (host memory, [n][2][4] u64 canonical affine) uploaded to `device` once and kept in the form the MSM reads.
+ * prime_id names the scalar field; only CW_PRIME_BN128 (BN254 G1) is accepted, anything else is CW_EINVAL.
+ * Every point must be (0, 0) or have both coordinates below q and lie on the curve; otherwise CW_EINVAL, and
+ * cw_last_error names the first bad index.  These checks run on the host before any device is touched.
+ * 1 <= n <= 2^26.  No device: CW_ENODEV. */
+int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g1_bases **out);
+void cw_g1_bases_destroy(cw_g1_bases *b);
+/* device scratch that cw_g1_msm_batch needs for `count` scalar vectors (it works through them in chunks, so the size
+ * stops growing with count beyond a chunk of about 2 GB) */
+int cw_g1_msm_scratch_bytes(const cw_g1_bases *b, uint32_t count, uint64_t *bytes);
+/* out_dev[c] = sum_{i<n} s_{c,i} P_i for c < count, affine canonical ([count][2][4] u64, (0,0) = infinity).
+ * The scalars of vector c are at scalars_dev + c * stride_elems * 4 (stride_elems >= n; 32-byte aligned).
+ * This is the layout of cw_r1cs_quotient_batch's h ([count][2^k][4]) and of cw_batch_expand_witness's rows.
+ * All pointers are device memory owned by the caller, 32-byte aligned, on the handle's device.  Asynchronous on `stream`
+ * (cudaStream_t as void*, NULL = the legacy default stream), so a call on cw_batch_stream(b) is ordered after the
+ * quotient or expansion that wrote the scalars. */
+int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                    uint64_t *out_dev, void *scratch_dev, void *stream);
+
 /* ---- multi-GPU: one process per GPU, independent inputs sharded over the ranks ---------------------------
  * The reference has no distributed mode (Circom_CalcWit is per-process state, calcwit.cpp:26-45).  Here rank 0
  * lowers the circuit and broadcasts the lowered form once; every rank runs its shard; witnesses are gathered in

@@ -1,0 +1,201 @@
+#!/usr/bin/env python
+"""Time the G1 multi-scalar multiplication (cw_g1_msm_batch) and the headline prover pipeline (quotient + H MSM).
+
+Prints, per shape, ms per MSM (CUDA events after a warm-up of that shape) and a lower bound: Montgomery products the
+chosen plan performs whatever the scalars (counted below from n, c, the scalars' nonzero digits and the formula costs of
+csrc/msm.cuh) over the product rate cw_fr_mul_bench measures in the same call.  That probe is built for bn128's scalar field; the MSM multiplies
+in the base field q, which has the same 254-bit size and the same product code, so the bn128 rate stands in for it.
+Scalar kinds: uniform random 256-bit values, and expanded Sha256compression witness rows tiled to n (mostly bits).
+The card's name, power limit and SM clock are read in the same call.  One JSON object per line.
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes
+import json
+import os
+import random
+import subprocess
+import sys
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+MADD, DBL = 10, 9   # Montgomery products of madd-2008-s and dbl-2008-s-1 as msm.cuh computes them
+
+
+def windows(c):
+    return 256 // c + 1
+
+
+def window_bits(n):
+    """msm_window_bits: the c in [2, 18] minimising W (n + 6 * 2^(c-1))"""
+    return min(range(2, 19), key=lambda c: (windows(c) * (n + 6 * (1 << (c - 1))), c))
+
+
+def nonzero_digits(s: int, c: int) -> int:
+    nz, carry = 0, 0
+    for _ in range(windows(c)):
+        raw = (s & ((1 << c) - 1)) + carry
+        s >>= c
+        carry = 1 if raw > (1 << (c - 1)) else 0
+        nz += (raw - (carry << c)) != 0
+    return nz
+
+
+def products(n, c, live):
+    """per MSM, the products every input performs: one mixed addition per live (point, window) item except the first of
+    each bucket (at most 2^(c-1) per window), and Horner's doublings.  The partial-sum levels and the bucket reduction are
+    left out: empty buckets and slots cost nothing, so their share depends on the scalars - the bound stays a bound"""
+    W, B = windows(c), 1 << (c - 1)
+    return max(0, live - W * B) * MADD + (W - 1) * c * DBL
+
+
+def card():
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True)
+    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unknown"
+
+
+def mont_rate(native) -> float:
+    n, iters = 132 * 2048 * 4, 2000
+    ms = ctypes.c_float()
+    native.check(native.lib.cw_fr_mul_bench(0, n, iters, 0, ctypes.byref(ms)))
+    return n * iters / (ms.value / 1e3)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--logs", default="16,20,21")
+    ap.add_argument("--counts", default="1,8,32")
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--sweep", default="20:14-19,21:15-19", help="log2 n:c range pairs timed at count 8, uniform scalars")
+    ap.add_argument("--pipeline", type=int, default=64, help="headline witnesses for quotient + H MSM (0: skip)")
+    args = ap.parse_args()
+    import torch
+    from circom_b200 import native
+    from circom_b200.circuit import CircuitDesc
+    from circom_b200 import circuits as C
+    from circom_b200.witness_calculator import Circuit, Batch, G1Bases, R1cs, limbs_to_ints
+    from oracle import g1_model as GM
+
+    rate = mont_rate(native)
+    print(json.dumps({"card": card(), "mont_products_per_s": rate, "rate_prime": "bn128"}), flush=True)
+    logs = [int(x) for x in args.logs.split(",")]
+    counts = [int(x) for x in args.counts.split(",")]
+    n_max = 1 << max(logs + [21])
+    rng = random.Random(1)
+    pts, _ = GM.multiples(rng.randrange(GM.R), rng.randrange(GM.R), n_max)
+    pts_np = np.frombuffer(b"".join(x.to_bytes(32, "little") + y.to_bytes(32, "little") for x, y in pts),
+                           dtype=np.uint64).reshape(-1, 2, 4)
+    del pts
+
+    # bit-heavy rows: expanded Sha256compression witnesses
+    d = CircuitDesc("bn128")
+    d.set_main(C.sha256_compression(d))
+    sc = Circuit(d, fuse=True)
+    sb = Batch(sc, max(counts))
+    ins = np.zeros((max(counts), sc.n_inputs, 4), dtype=np.uint64)
+    ins[:, :, 0] = np.random.default_rng(0).integers(0, 2, size=(max(counts), sc.n_inputs), dtype=np.uint64)
+    sb.set_inputs(ins)
+    sb.run()
+    wrows = sb.witness()
+    del sb
+
+    def time_msm(b, s, n, cnt):
+        out = torch.zeros((cnt, 2, 4), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(b.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.reps):
+            b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / args.reps
+
+    for k in logs:
+        n = 1 << k
+        b = G1Bases(pts_np[:n])
+        c = window_bits(n)
+        for kind in ("uniform", "bits"):
+            for cnt in counts:
+                if kind == "uniform":
+                    s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+                    live = cnt * n * windows(c)   # (nonzero digits of uniform scalars: all but a 2^-c fraction)
+                else:
+                    reps = -(-n // wrows.shape[1])
+                    host = np.concatenate([np.tile(wrows[i % wrows.shape[0]], (reps, 1))[:n][None] for i in range(cnt)])
+                    s = torch.from_numpy(host.view(np.int64)).cuda()
+                    live = 0
+                    for i in range(cnt):
+                        row = limbs_to_ints(wrows[i % wrows.shape[0]])
+                        per = sum(nonzero_digits(v, c) for v in row)
+                        full, part = divmod(n, len(row))
+                        live += full * per + sum(nonzero_digits(v, c) for v in row[:part])
+                ms = time_msm(b, s, n, cnt)
+                pr = products(n, c, live // cnt)
+                lb = pr / rate * 1e3
+                print(json.dumps({"what": "g1_msm", "scalars": kind, "log2_n": k, "c": c, "count": cnt, "ms_call": round(ms, 3),
+                                  "ms_per_msm": round(ms / cnt, 3), "mont_products_per_msm": pr,
+                                  "lower_bound_ms_per_msm": round(lb, 3), "x_bound": round(ms / cnt / lb, 2)}), flush=True)
+                del s
+                torch.cuda.empty_cache()
+        del b
+
+    # window sweep
+    for part in filter(None, args.sweep.split(",")):
+        k, rng_c = part.split(":")
+        lo, hi = (int(x) for x in rng_c.split("-"))
+        n, cnt = 1 << int(k), 8
+        b = G1Bases(pts_np[:n])
+        s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+        for c in range(lo, hi + 1):
+            os.environ["CW_MSM_WINDOW"] = str(c)
+            ms = time_msm(b, s, n, cnt)
+            print(json.dumps({"what": "window_sweep", "log2_n": int(k), "c": c, "rule_c": window_bits(n), "count": cnt,
+                              "ms_per_msm": round(ms / cnt, 3)}), flush=True)
+        os.environ.pop("CW_MSM_WINDOW", None)
+        del b, s
+        torch.cuda.empty_cache()
+
+    # the headline pipeline: quotient of `pipeline` witnesses, then their H MSMs on the batch stream
+    if args.pipeline:
+        cnt = args.pipeline
+        d = CircuitDesc("bn128")
+        d.set_main(C.ecdsa_scale(d, 8, 132))
+        r_ = np.random.default_rng(0)
+        ins = np.zeros((cnt, d.main.n_in, 4), dtype=np.uint64)
+        ins[:, :, 0] = r_.integers(0, 2**64, size=(cnt, d.main.n_in), dtype=np.uint64)
+        c = Circuit(d, fuse=True)
+        bt = Batch(c, cnt)
+        bt.set_inputs(ins)
+        bt.run()
+        r = R1cs(c)
+        k, _ = r.qap_info()
+        n = 1 << k
+        g = G1Bases(pts_np[:n])
+        stream = torch.cuda.ExternalStream(bt.stream())
+        h = torch.empty((cnt, n, 4), dtype=torch.int64, device="cuda")
+        qs = torch.empty((2 * cnt, n, 4), dtype=torch.int64, device="cuda")
+        out = torch.zeros((cnt, 2, 4), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(g.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        for rep in range(2):   # the first round is the warm-up
+            ev[0].record(stream)
+            r.quotient_batch(bt, 0, cnt, h.data_ptr(), qs.data_ptr())
+            ev[1].record(stream)
+            g.msm(h.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr(), bt.stream())
+            ev[2].record(stream)
+            bt.sync()
+        q_ms, m_ms = ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])
+        print(json.dumps({"what": "pipeline", "log2_n": k, "witnesses": cnt, "quotient_ms_per_witness": round(q_ms / cnt, 3),
+                          "h_msm_ms_per_witness": round(m_ms / cnt, 3),
+                          "total_ms_per_witness": round((q_ms + m_ms) / cnt, 3)}), flush=True)
+    print(json.dumps({"card_after": card()}), flush=True)
+
+
+if __name__ == "__main__":
+    main()
