@@ -8,9 +8,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcircom_b200.so")
 CLI = os.path.join(HERE, "circom_cuda_witness")
-SOURCES = ["capi.cu", "tape_calls.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
+SOURCES = ["capi.cu", "tape_calls.cu", "msm_g2.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
 CLI_SOURCES = ["cli.cpp"]
-HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
+HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "msm_g2.cuh", "msm_g2.h", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 

@@ -27,6 +27,7 @@
 
 #include "kernels.cuh"
 #include "msm.cuh"
+#include "msm_g2.h"
 #include "tape_calls.h"
 #include "tape.h"
 #include "hostpack.h"
@@ -88,6 +89,7 @@ int ensure_device(int device) {
         for (int k = 0; k < N_PRIMES_DEV; ++k) h[k] = make_dev_params(make_field(k));
         CU(cudaMemcpyToSymbol(c_fr, h, sizeof(h)));
         CU(tape_calls_set_params(h, sizeof(h)));
+        CU(msm_g2_set_params(h, sizeof(h)));
         g_dev_ready[device] = true;
     }
     return CW_OK;
@@ -1845,7 +1847,8 @@ static u32 msm_seg_bits(u32 segs) {   // bits of the largest segment index
     while (b < 32 && ((uint64_t)1 << b) < segs) ++b;
     return b;
 }
-static int msm_plan(uint64_t n, u32 chunk, MsmPlan &p) {
+// pt_bytes: the bucket type's size, sizeof(Xyzz) for G1 and MSM_G2_POINT_BYTES for G2
+static int msm_plan(uint64_t n, u32 chunk, MsmPlan &p, size_t pt_bytes) {
     p.n = n;
     const int cw = env_int("CW_MSM_WINDOW", 0);   // (window sweeps: scripts/msm_bench.py)
     p.c = cw >= (int)MSM_MIN_C && cw <= (int)MSM_MAX_C ? (u32)cw : msm_window_bits(n);
@@ -1868,27 +1871,27 @@ static int msm_plan(uint64_t n, u32 chunk, MsmPlan &p) {
         p.vals[k] = take(p.items * 4);
     }
     p.cub = take(p.cub_bytes);
-    p.buckets = take((size_t)chunk * p.W * p.B * sizeof(Xyzz));
+    p.buckets = take((size_t)chunk * p.W * p.B * pt_bytes);
     for (int k = 0; k < 2; ++k) {
         p.lv_keys[k] = take(p.slots[k] * 4);
-        p.lv_pts[k] = take(p.slots[k] * sizeof(Xyzz));
+        p.lv_pts[k] = take(p.slots[k] * pt_bytes);
     }
     const u32 m = p.B < MSM_SEG ? p.B : MSM_SEG;
-    p.segs = take((size_t)chunk * p.W * (p.B / m) * sizeof(Xyzz));
-    p.wins = take((size_t)chunk * p.W * sizeof(Xyzz));
+    p.segs = take((size_t)chunk * p.W * (p.B / m) * pt_bytes);
+    p.wins = take((size_t)chunk * p.W * pt_bytes);
     p.total = at;
     return CW_OK;
 }
 // the chunk size for `count` instances of n points: bounded by MSM_CHUNK_BYTES, the 32-bit keys and int item counts
-static int msm_plan_for(uint64_t n, u32 count, MsmPlan &p) {
+static int msm_plan_for(uint64_t n, u32 count, MsmPlan &p, size_t pt_bytes = sizeof(Xyzz)) {
     MsmPlan one;
-    int rc = msm_plan(n, 1, one);
+    int rc = msm_plan(n, 1, one, pt_bytes);
     if (rc) return rc;
     uint64_t chunk = std::max<uint64_t>(1, MSM_CHUNK_BYTES / one.total);
     chunk = std::min<uint64_t>(chunk, count);
     chunk = std::min<uint64_t>(chunk, ((1ull << (32 - one.c)) - 1) / one.W);
     chunk = std::min<uint64_t>(chunk, std::max<uint64_t>(1, (uint64_t)INT32_MAX / (one.W * n)));
-    return msm_plan(n, (u32)chunk, p);
+    return msm_plan(n, (u32)chunk, p, pt_bytes);
 }
 
 int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g1_bases **out) {
@@ -1945,14 +1948,16 @@ int cw_g1_msm_scratch_bytes(const cw_g1_bases *b, uint32_t count, uint64_t *byte
     return CW_OK;
 }
 
-int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
-                    uint64_t *out_dev, void *scratch_dev, void *stream) {
-    if (!b || !scalars_dev || !out_dev || !scratch_dev || count == 0) return fail(CW_EINVAL, "bad argument");
-    if (stride_elems < b->n) return fail(CW_EINVAL, "stride_elems must be at least the number of points");
+// the argument checks of cw_g1_msm_batch / cw_g2_msm_batch that need no device; then the device pointers
+static int msm_check_args(uint64_t n, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count, uint64_t *out_dev,
+                          void *scratch_dev) {
+    if (!scalars_dev || !out_dev || !scratch_dev || count == 0) return fail(CW_EINVAL, "bad argument");
+    if (stride_elems < n) return fail(CW_EINVAL, "stride_elems must be at least the number of points");
     if (((uintptr_t)scalars_dev | (uintptr_t)out_dev | (uintptr_t)scratch_dev) & 31u)
         return fail(CW_EINVAL, "device pointers must be 32-byte aligned");
-    int rc = ensure_device(b->device);
-    if (rc) return rc;
+    return CW_OK;
+}
+static int msm_check_pointers(int device, const uint64_t *scalars_dev, uint64_t *out_dev, void *scratch_dev) {
     for (const void *p : {(const void *)scalars_dev, (const void *)out_dev, (const void *)scratch_dev}) {
         cudaPointerAttributes a;
         if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -1960,23 +1965,44 @@ int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride
             return fail(CW_EINVAL, "not a device pointer");
         }
         if (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) return fail(CW_EINVAL, "not device memory");
-        if (a.device != b->device) return fail(CW_EINVAL, "device memory of another device than the bases'");
+        if (a.device != device) return fail(CW_EINVAL, "device memory of another device than the bases'");
     }
+    return CW_OK;
+}
+
+// the digits of instances [i0, i0 + cn) and their sort: sorted keys and values in the plan's keys[1] / vals[1].  The same
+// for G1 and G2: the digits do not depend on the group.
+static int msm_sorted_digits(const MsmPlan &p, char *S, const uint64_t *scalars_dev, uint64_t stride_elems, u32 n, u32 i0,
+                             u32 cn, cudaStream_t st) {
+    const u32 n_win = cn * p.W, sms = device_sms();
+    const uint64_t N = (uint64_t)n_win * n;
+    u32 *k0 = (u32 *)(S + p.keys[0]), *k1 = (u32 *)(S + p.keys[1]), *v0 = (u32 *)(S + p.vals[0]), *v1 = (u32 *)(S + p.vals[1]);
+    dim3 grid(std::max<u32>(1, std::min<u32>((n + MSM_THREADS - 1) / MSM_THREADS, sms * 8)), std::min<u32>(cn, 65535u));
+    msm_digits_kernel<<<grid, MSM_THREADS, 0, st>>>((const uint4 *)(scalars_dev + 4 * (size_t)i0 * stride_elems),
+                                                    stride_elems, n, p.c, p.W, cn, k0, v0);
+    size_t cub_bytes = p.cub_bytes;
+    CU(cub::DeviceRadixSort::SortPairs(S + p.cub, cub_bytes, k0, k1, v0, v1, (int)N, 0, (int)(p.c + msm_seg_bits(n_win)), st));
+    return CW_OK;
+}
+
+int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                    uint64_t *out_dev, void *scratch_dev, void *stream) {
+    if (!b) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(b->n, scalars_dev, stride_elems, count, out_dev, scratch_dev);
+    if (rc) return rc;
+    if ((rc = ensure_device(b->device))) return rc;
+    if ((rc = msm_check_pointers(b->device, scalars_dev, out_dev, scratch_dev))) return rc;
     MsmPlan p;
     if ((rc = msm_plan_for(b->n, count, p))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     char *S = (char *)scratch_dev;
-    const u32 n = (u32)b->n, sms = device_sms();
+    const u32 n = (u32)b->n;
     const u32 m = p.B < MSM_SEG ? p.B : MSM_SEG, per = p.B / m;
     for (u32 i0 = 0; i0 < count; i0 += p.chunk) {
         const u32 cn = std::min(p.chunk, count - i0), n_win = cn * p.W;
         const uint64_t N = (uint64_t)n_win * n;
-        u32 *k0 = (u32 *)(S + p.keys[0]), *k1 = (u32 *)(S + p.keys[1]), *v0 = (u32 *)(S + p.vals[0]), *v1 = (u32 *)(S + p.vals[1]);
-        dim3 grid(std::max<u32>(1, std::min<u32>((n + MSM_THREADS - 1) / MSM_THREADS, sms * 8)), std::min<u32>(cn, 65535u));
-        msm_digits_kernel<<<grid, MSM_THREADS, 0, st>>>((const uint4 *)(scalars_dev + 4 * (size_t)i0 * stride_elems),
-                                                        stride_elems, n, p.c, p.W, cn, k0, v0);
-        size_t cub_bytes = p.cub_bytes;
-        CU(cub::DeviceRadixSort::SortPairs(S + p.cub, cub_bytes, k0, k1, v0, v1, (int)N, 0, (int)(p.c + msm_seg_bits(n_win)), st));
+        if ((rc = msm_sorted_digits(p, S, scalars_dev, stride_elems, n, i0, cn, st))) return rc;
+        const u32 *k1 = (const u32 *)(S + p.keys[1]), *v1 = (const u32 *)(S + p.vals[1]);
         Xyzz *buckets = (Xyzz *)(S + p.buckets);
         CU(cudaMemsetAsync(buckets, 0, (size_t)n_win * p.B * sizeof(Xyzz), st));
         // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
@@ -1998,6 +2024,127 @@ int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride
         msm_windows_kernel<<<n_win, MSM_THREADS, 0, st>>>(segs, per, wins);
         msm_final_kernel<<<(cn + MSM_THREADS - 1) / MSM_THREADS, MSM_THREADS, 0, st>>>(wins, p.W, p.c, cn,
                                                                                       (uint4 *)(out_dev + 8 * (size_t)i0));
+        CU(cudaGetLastError());
+    }
+    return CW_OK;
+}
+
+// ---- multi-scalar multiplication on G2 of BN254 (msm_g2.cuh, kernels in msm_g2.cu) ------------------------------------
+struct cw_g2_bases {
+    int device = 0;
+    uint64_t n = 0;
+    u32 *pts = nullptr;   // [n][32] u32: Montgomery x.c0, x.c1, y.c0, y.c1; all zeros = infinity
+};
+
+// b' = 3 / (9 + u), canonical (c0, c1)
+static const uint64_t G2_TWIST_B[2][4] = {
+    {0x3267e6dc24a138e5ull, 0xb5b4c5e559dbefa3ull, 0x81be18991be06ac3ull, 0x2b149d40ceb8aaaeull},
+    {0xe4a2bd0685c315d2ull, 0xa74fa084e52d1852ull, 0xcd2cafadeed8fdf4ull, 0x009713b03af0fed4ull},
+};
+
+int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g2_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G2 bases are built for bn128 (BN254) only");
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    const FieldParams F = make_field(MSM_PRIME);
+    // Fq2 on the host, Montgomery images (c0, c1): the check y^2 = x^3 + b' is written apart from the device formulas
+    struct E2 { U256 c0, c1; };
+    auto mul = [&](const E2 &a, const E2 &b) {
+        const U256 t0 = F.mont_mul(a.c0, b.c0), t1 = F.mont_mul(a.c1, b.c1);
+        const U256 m = F.mont_mul(F.addm(a.c0, a.c1), F.addm(b.c0, b.c1));
+        return E2{F.subm(t0, t1), F.subm(F.subm(m, t0), t1)};
+    };
+    U256 b0, b1;
+    memcpy(b0.v, G2_TWIST_B[0], 32);
+    memcpy(b1.v, G2_TWIST_B[1], 32);
+    const E2 bt{F.to_mont(b0), F.to_mont(b1)};
+    std::vector<U256> mont(4 * n);
+    for (uint64_t i = 0; i < n; ++i) {
+        U256 c[4];
+        bool zero = true;
+        for (int k = 0; k < 4; ++k) {
+            memcpy(c[k].v, points + 16 * i + 4 * k, 32);
+            zero = zero && c[k].is_zero();
+        }
+        if (zero) {
+            for (int k = 0; k < 4; ++k) mont[4 * i + k] = c[k];
+            continue;
+        }
+        for (int k = 0; k < 4; ++k)
+            if (!(c[k] < F.q))
+                return fail(CW_EINVAL, "point " + std::to_string(i) + ": coefficient " + std::to_string(k) +
+                                           " (x.c0, x.c1, y.c0, y.c1) is not below q");
+        const E2 x{F.to_mont(c[0]), F.to_mont(c[1])}, y{F.to_mont(c[2]), F.to_mont(c[3])};
+        const E2 yy = mul(y, y), xxx = mul(mul(x, x), x);
+        if (yy.c0 != F.addm(xxx.c0, bt.c0) || yy.c1 != F.addm(xxx.c1, bt.c1))
+            return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the twist y^2 = x^3 + 3 / (9 + u)");
+        mont[4 * i] = x.c0;
+        mont[4 * i + 1] = x.c1;
+        mont[4 * i + 2] = y.c0;
+        mont[4 * i + 3] = y.c1;
+    }
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    cw_g2_bases *b = new cw_g2_bases();
+    b->device = device;
+    b->n = n;
+    if ((rc = upload(&b->pts, mont.data(), (size_t)n * 128))) {
+        delete b;
+        return rc;
+    }
+    *out = b;
+    return CW_OK;
+}
+
+void cw_g2_bases_destroy(cw_g2_bases *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    cudaFree(b->pts);
+    delete b;
+}
+
+int cw_g2_msm_scratch_bytes(const cw_g2_bases *b, uint32_t count, uint64_t *bytes) {
+    if (!b || !bytes || count == 0) return fail(CW_EINVAL, "bad argument");
+    int rc = ensure_device(b->device);
+    if (rc) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_G2_POINT_BYTES))) return rc;
+    *bytes = p.total;
+    return CW_OK;
+}
+
+int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                    uint64_t *out_dev, void *scratch_dev, void *stream) {
+    if (!b) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(b->n, scalars_dev, stride_elems, count, out_dev, scratch_dev);
+    if (rc) return rc;
+    if ((rc = ensure_device(b->device))) return rc;
+    if ((rc = msm_check_pointers(b->device, scalars_dev, out_dev, scratch_dev))) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_G2_POINT_BYTES))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char *S = (char *)scratch_dev;
+    const u32 n = (u32)b->n;
+    for (u32 i0 = 0; i0 < count; i0 += p.chunk) {
+        const u32 cn = std::min(p.chunk, count - i0), n_win = cn * p.W;
+        const uint64_t N = (uint64_t)n_win * n;
+        if ((rc = msm_sorted_digits(p, S, scalars_dev, stride_elems, n, i0, cn, st))) return rc;
+        void *buckets = S + p.buckets;
+        CU(cudaMemsetAsync(buckets, 0, (size_t)n_win * p.B * MSM_G2_POINT_BYTES, st));
+        // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
+        uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
+        int lv = 0;
+        msm_g2_launch_runs(true, (const u32 *)(S + p.keys[1]), (const u32 *)(S + p.vals[1]), b->pts, nullptr, N, p.c, buckets,
+                           (u32 *)(S + p.lv_keys[0]), S + p.lv_pts[0], st);
+        while (threads > 1) {
+            items = msm_level_out(items);
+            threads = (items + MSM_RUN - 1) / MSM_RUN;
+            msm_g2_launch_runs(false, (const u32 *)(S + p.lv_keys[lv]), nullptr, nullptr, S + p.lv_pts[lv], items, p.c, buckets,
+                               (u32 *)(S + p.lv_keys[lv ^ 1]), S + p.lv_pts[lv ^ 1], st);
+            lv ^= 1;
+        }
+        msm_g2_launch_reduce(buckets, p.B, n_win, S + p.segs, S + p.wins, p.W, p.c, cn, (uint4 *)(out_dev + 16 * (size_t)i0), st);
         CU(cudaGetLastError());
     }
     return CW_OK;

@@ -136,8 +136,10 @@ CW_HD void xyzz_add(Xyzz &a, const Xyzz &b, const FrParams &P) {
     fr_sub(a.y, q, t, P);               // Y3 = R (Q - X3) - S1 PPP
 }
 
-// r = k p for a small k (double-and-add from the top bit)
-CW_HD void xyzz_mul_small(Xyzz &r, const Xyzz &p, u32 k, const FrParams &P) {
+// r = k p for a small k (double-and-add from the top bit); Pt: Xyzz here, XyzzG2 in msm_g2.cuh (the point functions are
+// found by overloading)
+template <class Pt>
+CW_HD void xyzz_mul_small(Pt &r, const Pt &p, u32 k, const FrParams &P) {
     xyzz_inf(r);
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
@@ -232,13 +234,17 @@ struct MsmXyzzItems {
 };
 
 // one run's sum at the end of a thread's range walk: a whole bucket goes to `buckets`, a run that continues past the
-// range goes to the thread's slot (first run: slot 0, last run: slot 1)
-struct MsmRunOut {
-    Xyzz *buckets;
+// range goes to the thread's slot (first run: slot 0, last run: slot 1).  The run machinery below does not depend on the
+// group: Pt is the bucket type (Xyzz for G1, XyzzG2 for G2 in msm_g2.cuh).
+template <class Pt>
+struct MsmRunOutT {
+    Pt *buckets;
     u32 *okeys;
-    Xyzz *opts;
+    Pt *opts;
 };
-CW_HD void msm_emit(const MsmRunOut &o, uint64_t t, u32 c, u32 key, const Xyzz &acc, bool first, bool last, u32 before,
+using MsmRunOut = MsmRunOutT<Xyzz>;
+template <class Pt>
+CW_HD void msm_emit(const MsmRunOutT<Pt> &o, uint64_t t, u32 c, u32 key, const Pt &acc, bool first, bool last, u32 before,
                     u32 after, u32 *slot_key) {
     if (!msm_live(key, c)) return;
     const bool open = (first && key == before) || (last && key == after);
@@ -248,7 +254,7 @@ CW_HD void msm_emit(const MsmRunOut &o, uint64_t t, u32 c, u32 key, const Xyzz &
         o.opts[2 * t] = acc;
         slot_key[0] = key;
         if (last) {   // the range is one run: slot 1 keeps the key (partials of a key stay adjacent) with nothing in it
-            Xyzz z;
+            Pt z;
             xyzz_inf(z);
             o.opts[2 * t + 1] = z;
             slot_key[1] = key;
@@ -260,14 +266,14 @@ CW_HD void msm_emit(const MsmRunOut &o, uint64_t t, u32 c, u32 key, const Xyzz &
 }
 
 // thread t of a level over N sorted items: sums the runs of [t MSM_RUN, (t + 1) MSM_RUN)
-template <class Items>
-CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const MsmRunOut &o, const FrParams &P) {
+template <class Items, class Pt>
+CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const MsmRunOutT<Pt> &o, const FrParams &P) {
     const uint64_t lo = t * MSM_RUN, hi = lo + MSM_RUN < N ? lo + MSM_RUN : N;
     const u32 before = lo > 0 ? it.keys[lo - 1] : MSM_NONE, after = hi < N ? it.keys[hi] : MSM_NONE;
     u32 slot_key[2] = {MSM_NONE, MSM_NONE};
     u32 cur = it.keys[lo];
     bool first = true;
-    Xyzz acc;
+    Pt acc;
     xyzz_inf(acc);
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
@@ -291,8 +297,9 @@ CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const Ms
 CW_HD uint64_t msm_level_out(uint64_t N) { return 2 * ((N + MSM_RUN - 1) / MSM_RUN); }
 
 // buckets [lo, lo + m) of one window (bucket b holds digit b + 1): sum_{b} (b + 1) B_b over the segment
-CW_HD void msm_bucket_segment(Xyzz &out, const Xyzz *win, u32 lo, u32 m, const FrParams &P) {
-    Xyzz run, tot, b;
+template <class Pt>
+CW_HD void msm_bucket_segment(Pt &out, const Pt *win, u32 lo, u32 m, const FrParams &P) {
+    Pt run, tot, b;
     xyzz_inf(run);
     xyzz_inf(tot);
 #if defined(__CUDA_ARCH__)
@@ -308,14 +315,15 @@ CW_HD void msm_bucket_segment(Xyzz &out, const Xyzz *win, u32 lo, u32 m, const F
 }
 
 // sum_w 2^(c w) S_w (Horner's rule from the top window)
-CW_HD void msm_horner(Xyzz &acc, const Xyzz *win, u32 W, u32 c, const FrParams &P) {
+template <class Pt>
+CW_HD void msm_horner(Pt &acc, const Pt *win, u32 W, u32 c, const FrParams &P) {
     msm_ld_xyzz(acc, win + (W - 1));
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif
     for (u32 w = W - 1; w-- > 0;) {
         for (u32 k = 0; k < c; ++k) xyzz_dbl(acc, P);
-        Xyzz s;
+        Pt s;
         msm_ld_xyzz(s, win + w);
         xyzz_add(acc, s, P);
     }
@@ -330,6 +338,10 @@ CW_HD void msm_horner(Xyzz &acc, const Xyzz *win, u32 W, u32 c, const FrParams &
 namespace cw {
 
 constexpr u32 MSM_THREADS = 256;
+
+// (the G2 unit, msm_g2.cu, includes this header for the shared functions and defines CW_MSM_NO_G1_KERNELS: the
+// non-template kernels must exist in one translation unit only)
+#ifndef CW_MSM_NO_G1_KERNELS
 
 // keys and values of `count` instances: item (instance i, window w, point j) at (i W + w) n + j.  grid.y = instances.
 __global__ void __launch_bounds__(MSM_THREADS) msm_digits_kernel(const uint4 *__restrict__ scalars, uint64_t stride_elems,
@@ -416,6 +428,7 @@ __global__ void __launch_bounds__(MSM_THREADS) msm_final_kernel(const Xyzz *__re
     stg256(out + 4 * (size_t)i, cx);
     stg256(out + 4 * (size_t)i + 2, cy);
 }
+#endif  // CW_MSM_NO_G1_KERNELS
 
 }  // namespace cw
 #endif

@@ -94,6 +94,10 @@ def _load() -> ctypes.CDLL:
         "cw_g1_bases_destroy": (None, [P]),
         "cw_g1_msm_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
         "cw_g1_msm_batch": (c_int, [P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_g2_bases_create": (c_int, [c_int, c_void_p, c_uint64, c_int, POINTER(P)]),
+        "cw_g2_bases_destroy": (None, [P]),
+        "cw_g2_msm_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
+        "cw_g2_msm_batch": (c_int, [P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
         "cw_comm_unique_id": (c_int, [c_void_p]),
         "cw_comm_init": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),
         "cw_comm_from_nccl": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),

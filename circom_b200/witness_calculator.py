@@ -558,6 +558,62 @@ class G1Bases:
         return [None if (x, y) == (0, 0) else (x, y) for x, y in zip(v[0::2], v[1::2])]
 
 
+class G2Bases:
+    """BN254 G2 points (on the twist over Fq2) on the device for multi-scalar multiplications (cw_g2_bases_*,
+    include/circom_b200.h).  points: numpy uint64 [n][2][2][4] canonical affine (x.c0, x.c1, y.c0, y.c1), or a list of
+    ((x0, x1), (y0, y1)) ints; all zeros or None is the point at infinity.  Points are checked to lie on the twist, not
+    to lie in the order-r subgroup."""
+
+    def __init__(self, points, device: int = 0, prime_id: int = 0):   # (the scalar field: bn128 is the only one)
+        if isinstance(points, np.ndarray):
+            arr = np.ascontiguousarray(points, dtype=np.uint64).reshape(-1, 2, 2, 4)
+        else:
+            arr = np.zeros((len(points), 2, 2, 4), dtype=np.uint64)
+            for i, p in enumerate(points):
+                for j, e in enumerate(((0, 0), (0, 0)) if p is None else p):
+                    for k, v in enumerate(e):
+                        arr[i, j, k] = [(v >> (64 * m)) & 0xFFFFFFFFFFFFFFFF for m in range(4)]
+        self.n = arr.shape[0]
+        self.device = device
+        self._h = ctypes.c_void_p()
+        check(lib.cw_g2_bases_create(prime_id, arr.ctypes.data, self.n, device, ctypes.byref(self._h)))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            lib.cw_g2_bases_destroy(h)
+
+    def scratch_bytes(self, count: int) -> int:
+        b = ctypes.c_uint64()
+        check(lib.cw_g2_msm_scratch_bytes(self._h, count, ctypes.byref(b)))
+        return b.value
+
+    def msm(self, scalars_ptr: int, stride: int, count: int, out_ptr: int, scratch_ptr: int, stream=None) -> None:
+        """out[c] = sum_i s_{c,i} Q_i into device [count][2][2][4] uint64; scalars: device [count][stride][4] uint64.
+        Asynchronous on `stream` (a Batch.stream() value; None = the legacy default stream)."""
+        check(lib.cw_g2_msm_batch(self._h, ctypes.c_void_p(scalars_ptr), stride, count, ctypes.c_void_p(out_ptr),
+                                  ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream or None)))
+
+    def msm_host(self, scalars) -> List[Optional[tuple]]:
+        """the MSMs of host scalars ([count][n] ints, or numpy uint64 [count][n][4]): [((x0, x1), (y0, y1)) or None]"""
+        import torch
+        if isinstance(scalars, np.ndarray):
+            arr = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, self.n, 4)
+        else:
+            arr = np.array([[[(s >> (64 * k)) & 0xFFFFFFFFFFFFFFFF for k in range(4)] for s in row] for row in scalars],
+                           dtype=np.uint64).reshape(-1, self.n, 4)
+        count = arr.shape[0]
+        dev = torch.device("cuda", self.device)
+        s = torch.from_numpy(arr.view(np.int64)).to(dev)
+        out = torch.zeros((count, 2, 2, 4), dtype=torch.int64, device=dev)
+        scratch = torch.empty(self.scratch_bytes(count), dtype=torch.uint8, device=dev)
+        self.msm(s.data_ptr(), self.n, count, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize(dev)
+        v = limbs_to_ints(out.cpu().numpy().view(np.uint64))
+        return [None if not any(v[4 * i:4 * i + 4]) else ((v[4 * i], v[4 * i + 1]), (v[4 * i + 2], v[4 * i + 3]))
+                for i in range(count)]
+
+
 class WitnessCalculator:
     """`builder(code, options)` of witness_calculator.js:1-106, for a circuit description."""
 

@@ -324,6 +324,32 @@ int cw_g1_msm_scratch_bytes(const cw_g1_bases *b, uint32_t count, uint64_t *byte
 int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
                     uint64_t *out_dev, void *scratch_dev, void *stream);
 
+/* ---- multi-scalar multiplication on G2 ------------------------------------------------------------------------------
+ * The prover's B2 = sum_i w_i Q_i over the proving key's G2 points.
+ *   G2 of BN254 is taken on the twist E': y^2 = x^3 + b' over Fq2 = Fq[u] / (u^2 + 1), b' = 3 / (9 + u), q the base field
+ *   of G1.  The subgroup of order r is G2; #E'(Fq2) = r (2q - r).
+ *   A point at the ABI is affine, [2][2][4] u64 canonical: x.c0, x.c1, y.c0, y.c1 for x = x.c0 + x.c1 u and likewise y,
+ *   128 bytes per point.  c0 comes first, the order snarkjs' .zkey uses for Fq2 (byte compatibility with that format is
+ *   not verified here), not the (c1, c0) order of the EVM pairing precompile.  The point at infinity is all zeros, which
+ *   is not on E' (b' != 0), so the encoding is unambiguous.
+ *   Points are checked to lie on E', not to lie in the order-r subgroup (that costs a scalar multiplication per point).
+ *   The result is the exact sum sum_i s_i Q_i in E'(Fq2) for any points on E', with s_i taken as a 256-bit integer;
+ *   "s and s mod r give the same point" holds for points of the subgroup only.
+ * The calls mirror the G1 ones above. */
+typedef struct cw_g2_bases cw_g2_bases;
+/* n points (host memory, [n][2][2][4] u64 canonical affine) uploaded to `device` once.  prime_id names the scalar field;
+ * only CW_PRIME_BN128 is accepted.  Every point must be all zeros or have its four coefficients below q and lie on E';
+ * otherwise CW_EINVAL, and cw_last_error names the first bad index.  These checks run on the host before any device is
+ * touched.  1 <= n <= 2^26.  No device: CW_ENODEV. */
+int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g2_bases **out);
+void cw_g2_bases_destroy(cw_g2_bases *b);
+/* device scratch that cw_g2_msm_batch needs for `count` scalar vectors (chunks of about 2 GB, as for G1) */
+int cw_g2_msm_scratch_bytes(const cw_g2_bases *b, uint32_t count, uint64_t *bytes);
+/* out_dev[c] = sum_{i<n} s_{c,i} Q_i for c < count, affine canonical ([count][2][2][4] u64, all zeros = infinity).
+ * Scalars, strides, alignment, devices and streams as for cw_g1_msm_batch. */
+int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                    uint64_t *out_dev, void *scratch_dev, void *stream);
+
 /* ---- multi-GPU: one process per GPU, independent inputs sharded over the ranks ---------------------------
  * The reference has no distributed mode (Circom_CalcWit is per-process state, calcwit.cpp:26-45).  Here rank 0
  * lowers the circuit and broadcasts the lowered form once; every rank runs its shard; witnesses are gathered in

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Time the G1 multi-scalar multiplication (cw_g1_msm_batch) and the headline prover pipeline (quotient + H MSM).
+"""Time the G1 multi-scalar multiplication (cw_g1_msm_batch) and the headline prover pipeline (quotient + H MSM); with
+--group g2, the G2 one (cw_g2_msm_batch) and the B1 (G1) and B2 (G2) MSMs over expanded headline witness rows.
 
 Prints, per shape, ms per MSM (CUDA events after a warm-up of that shape) and a lower bound: Montgomery products the
 chosen plan performs whatever the scalars (counted below from n, c, the scalars' nonzero digits and the formula costs of
-csrc/msm.cuh) over the product rate cw_fr_mul_bench measures in the same call.  That probe is built for bn128's scalar field; the MSM multiplies
+csrc/msm.cuh, csrc/msm_g2.cuh: an Fq2 product is 3 products, a square 2) over the product rate cw_fr_mul_bench measures in the same call.  That probe is built for bn128's scalar field; the MSM multiplies
 in the base field q, which has the same 254-bit size and the same product code, so the bn128 rate stands in for it.
 Scalar kinds: uniform random 256-bit values, and expanded Sha256compression witness rows tiled to n (mostly bits).
 The card's name, power limit and SM clock are read in the same call.  One JSON object per line.
@@ -23,6 +24,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 MADD, DBL = 10, 9   # Montgomery products of madd-2008-s and dbl-2008-s-1 as msm.cuh computes them
+MADD_G2, DBL_G2 = 28, 24   # the same over Fq2 in msm_g2.cuh: 8 M + 2 S and 6 M + 3 S, M = 3 and S = 2 products
 
 
 def windows(c):
@@ -44,12 +46,12 @@ def nonzero_digits(s: int, c: int) -> int:
     return nz
 
 
-def products(n, c, live):
+def products(n, c, live, madd=MADD, dbl=DBL):
     """per MSM, the products every input performs: one mixed addition per live (point, window) item except the first of
     each bucket (at most 2^(c-1) per window), and Horner's doublings.  The partial-sum levels and the bucket reduction are
     left out: empty buckets and slots cost nothing, so their share depends on the scalars - the bound stays a bound"""
     W, B = windows(c), 1 << (c - 1)
-    return max(0, live - W * B) * MADD + (W - 1) * c * DBL
+    return max(0, live - W * B) * madd + (W - 1) * c * dbl
 
 
 def card():
@@ -72,7 +74,11 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--sweep", default="20:14-19,21:15-19", help="log2 n:c range pairs timed at count 8, uniform scalars")
     ap.add_argument("--pipeline", type=int, default=64, help="headline witnesses for quotient + H MSM (0: skip)")
+    ap.add_argument("--group", choices=("g1", "g2"), default="g1",
+                    help="g2: time cw_g2_msm_batch, and the pipeline leg is B1 + B2 over expanded headline witness rows")
     args = ap.parse_args()
+    if args.group == "g2":
+        return main_g2(args)
     import torch
     from circom_b200 import native
     from circom_b200.circuit import CircuitDesc
@@ -194,6 +200,141 @@ def main():
         print(json.dumps({"what": "pipeline", "log2_n": k, "witnesses": cnt, "quotient_ms_per_witness": round(q_ms / cnt, 3),
                           "h_msm_ms_per_witness": round(m_ms / cnt, 3),
                           "total_ms_per_witness": round((q_ms + m_ms) / cnt, 3)}), flush=True)
+    print(json.dumps({"card_after": card()}), flush=True)
+
+
+def main_g2(args):
+    import torch
+    from circom_b200 import native
+    from circom_b200.circuit import CircuitDesc
+    from circom_b200 import circuits as C
+    from circom_b200.witness_calculator import Circuit, Batch, G1Bases, G2Bases, limbs_to_ints
+    from oracle import g1_model as GM
+    from oracle import g2_model as M2
+
+    rate = mont_rate(native)
+    print(json.dumps({"card": card(), "mont_products_per_s": rate, "rate_prime": "bn128", "group": "g2"}), flush=True)
+    logs = [int(x) for x in args.logs.split(",")]
+    counts = [int(x) for x in args.counts.split(",")]
+    n_max = 1 << max(logs + [21])
+    rng = random.Random(1)
+    pts, _ = M2.multiples(rng.randrange(M2.R), rng.randrange(M2.R), n_max)
+    pts_np = np.frombuffer(b"".join(c.to_bytes(32, "little") for p in pts for e in p for c in e),
+                           dtype=np.uint64).reshape(-1, 2, 2, 4)
+    del pts
+
+    d = CircuitDesc("bn128")
+    d.set_main(C.sha256_compression(d))
+    sc = Circuit(d, fuse=True)
+    sb = Batch(sc, max(counts))
+    ins = np.zeros((max(counts), sc.n_inputs, 4), dtype=np.uint64)
+    ins[:, :, 0] = np.random.default_rng(0).integers(0, 2, size=(max(counts), sc.n_inputs), dtype=np.uint64)
+    sb.set_inputs(ins)
+    sb.run()
+    wrows = sb.witness()
+    del sb
+
+    def time_msm(b, s, n, cnt):
+        out = torch.zeros((cnt, 2, 2, 4), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(b.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.reps):
+            b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / args.reps
+
+    for k in logs:
+        n = 1 << k
+        b = G2Bases(pts_np[:n])
+        c = int(os.environ.get("CW_MSM_WINDOW", 0)) or window_bits(n)
+        for kind in ("uniform", "bits"):
+            for cnt in counts:
+                if kind == "uniform":
+                    s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+                    live = cnt * n * windows(c)
+                else:
+                    reps = -(-n // wrows.shape[1])
+                    host = np.concatenate([np.tile(wrows[i % wrows.shape[0]], (reps, 1))[:n][None] for i in range(cnt)])
+                    s = torch.from_numpy(host.view(np.int64)).cuda()
+                    live = 0
+                    for i in range(cnt):
+                        row = limbs_to_ints(wrows[i % wrows.shape[0]])
+                        per = sum(nonzero_digits(v, c) for v in row)
+                        full, part = divmod(n, len(row))
+                        live += full * per + sum(nonzero_digits(v, c) for v in row[:part])
+                ms = time_msm(b, s, n, cnt)
+                pr = products(n, c, live // cnt, MADD_G2, DBL_G2)
+                lb = pr / rate * 1e3
+                print(json.dumps({"what": "g2_msm", "scalars": kind, "log2_n": k, "c": c, "count": cnt, "ms_call": round(ms, 3),
+                                  "ms_per_msm": round(ms / cnt, 3), "mont_products_per_msm": pr,
+                                  "lower_bound_ms_per_msm": round(lb, 3), "x_bound": round(ms / cnt / lb, 2)}), flush=True)
+                del s
+                torch.cuda.empty_cache()
+        del b
+
+    for part in filter(None, args.sweep.split(",")):
+        k, rng_c = part.split(":")
+        lo, hi = (int(x) for x in rng_c.split("-"))
+        n, cnt = 1 << int(k), 8
+        b = G2Bases(pts_np[:n])
+        s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+        for c in range(lo, hi + 1):
+            os.environ["CW_MSM_WINDOW"] = str(c)
+            ms = time_msm(b, s, n, cnt)
+            print(json.dumps({"what": "window_sweep_g2", "log2_n": int(k), "c": c, "rule_c": window_bits(n), "count": cnt,
+                              "ms_per_msm": round(ms / cnt, 3)}), flush=True)
+        os.environ.pop("CW_MSM_WINDOW", None)
+        del b, s
+        torch.cuda.empty_cache()
+
+    # the headline pipeline leg: B1 (G1) and B2 (G2) over `pipeline` expanded headline witness rows, on the batch stream
+    if args.pipeline:
+        cnt = args.pipeline
+        d = CircuitDesc("bn128")
+        d.set_main(C.ecdsa_scale(d, 8, 132))
+        r_ = np.random.default_rng(0)
+        ins = np.zeros((cnt, d.main.n_in, 4), dtype=np.uint64)
+        ins[:, :, 0] = r_.integers(0, 2**64, size=(cnt, d.main.n_in), dtype=np.uint64)
+        c = Circuit(d, fuse=True)
+        bt = Batch(c, cnt)
+        bt.set_inputs(ins)
+        bt.run()
+        nw = c.n_witness
+        g1pts, _ = GM.multiples(rng.randrange(GM.R), rng.randrange(GM.R), nw)
+        g1 = G1Bases(np.frombuffer(b"".join(x.to_bytes(32, "little") + y.to_bytes(32, "little") for x, y in g1pts),
+                                   dtype=np.uint64).reshape(-1, 2, 4))
+        del g1pts
+        if nw > pts_np.shape[0]:
+            more, _ = M2.multiples(rng.randrange(M2.R), rng.randrange(M2.R), nw)
+            pts_np = np.frombuffer(b"".join(c.to_bytes(32, "little") for p in more for e in p for c in e),
+                                   dtype=np.uint64).reshape(-1, 2, 2, 4)
+            del more
+        g2 = G2Bases(pts_np[:nw])
+        stream = torch.cuda.ExternalStream(bt.stream())
+        rows = torch.empty((cnt, nw, 4), dtype=torch.int64, device="cuda")
+        o1 = torch.zeros((cnt, 2, 4), dtype=torch.int64, device="cuda")
+        o2 = torch.zeros((cnt, 2, 2, 4), dtype=torch.int64, device="cuda")
+        s1 = torch.empty(g1.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        s2 = torch.empty(g2.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        for rep in range(2):   # the first round is the warm-up
+            ev[0].record(stream)
+            bt.expand_witness(0, cnt, rows.data_ptr())
+            ev[1].record(stream)
+            g1.msm(rows.data_ptr(), nw, cnt, o1.data_ptr(), s1.data_ptr(), bt.stream())
+            ev[2].record(stream)
+            g2.msm(rows.data_ptr(), nw, cnt, o2.data_ptr(), s2.data_ptr(), bt.stream())
+            ev[3].record(stream)
+            bt.sync()
+        e_ms, b1_ms, b2_ms = (ev[i].elapsed_time(ev[i + 1]) for i in range(3))
+        print(json.dumps({"what": "pipeline_b1_b2", "n_witness": nw, "c": window_bits(nw), "witnesses": cnt,
+                          "expand_ms_per_witness": round(e_ms / cnt, 3), "b1_g1_msm_ms_per_witness": round(b1_ms / cnt, 3),
+                          "b2_g2_msm_ms_per_witness": round(b2_ms / cnt, 3),
+                          "b2_over_b1": round(b2_ms / b1_ms, 2)}), flush=True)
     print(json.dumps({"card_after": card()}), flush=True)
 
 
