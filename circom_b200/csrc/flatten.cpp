@@ -119,7 +119,7 @@ struct Val {
 // device-only opcodes (kernels.cuh / fr_device.cuh)
 enum { DOP_BITS = 29, DOP_ASSERT_BOOL = 30, DOP_MULSMALL = 31, DOP_BITSIP = 32, DOP_ASSERT_FITS = 33 };
 // width-classed forms (fr_device.cuh OP_ADDI ...): chosen when the tape word is written, from the static widths
-enum { DOP_ADDI = 48, DOP_SHRK = 49, DOP_SHLK = 50, DOP_ADDI_H = 52, DOP_MULI_Q = 53, DOP_MULI_H = 54, DOP_SHRK_H = 55,
+enum { DOP_ADDI = 48, DOP_SHRK = 49, DOP_SHLK = 50, DOP_MULK = 51, DOP_ADDI_H = 52, DOP_MULI_Q = 53, DOP_MULI_H = 54, DOP_SHRK_H = 55,
        DOP_SHLK_H = 56 };
 inline bool c_is_immediate(uint32_t opcode) {
     return opcode == CW_OP_ASSERT || opcode == CW_OP_ASSERT_EQ || opcode == DOP_BITS || opcode == DOP_ASSERT_BOOL ||
@@ -1753,6 +1753,30 @@ struct Lowerer {
                 default: return o[0];
             }
         };
+        // Products by small constants.  MontMul(x, K) = x K R^-1 = x k mod q with k = K R^-1 mod q, whatever the
+        // representation of x (a constant factor K = k R keeps x's form).  When k <= 2^64 the word becomes OP_MULK, which
+        // computes x k mod q by a Barrett reduction (fr_mul_small): the same residue for about a quarter of the work.
+        // Its b operand is a constant holding k and the prime's Barrett constant.  Those constants are added with
+        // CW_FLAG_NO_NARROW as well, where they go unused: the two tapes then differ in their words only.
+        struct MulK { uint32_t cls, operand; };   // cls: 1 k < 2^32, 2 k <= 2^64, 3 wider; operand: {k, mu} or NO_SLOT
+        std::unordered_map<uint32_t, MulK> mulk_of;    // by the constant-table index of K
+        const bool mulk_prime = F.qbits > 224;         // (fr_mul_small's limb positions; not goldilocks)
+        const uint64_t mu = mulk_prime ? F.barrett_mu() : 0;
+        auto mulk = [&](uint32_t i) -> MulK {
+            const uint32_t *o = &pops[(size_t)i * 4];
+            if (o[0] != CW_OP_MUL || o[2] == NO_SLOT || !(o[2] & OPERAND_CONST)) return MulK{0, NO_SLOT};
+            const uint32_t K = o[2] & 0x7FFFFFFFu;
+            auto it = mulk_of.find(K);
+            if (it != mulk_of.end()) return it->second;
+            const U256 k = F.from_mont(consts[K]);
+            MulK r{3, NO_SLOT};
+            if (!(k.v[1] | k.v[2] | k.v[3])) r.cls = k.v[0] >> 32 ? 2 : 1;
+            else if (k.v[1] == 1 && !k.v[0] && !(k.v[2] | k.v[3])) r.cls = 2;   // 2^64 (carry weights)
+            if (r.cls < 3 && mulk_prime) r.operand = OPERAND_CONST | raw_const(U256{{k.v[0], k.v[1], mu, 0}});
+            mulk_of.emplace(K, r);
+            return r;
+        };
+        uint64_t mul_census[4] = {0, 0, 0, 0};   // products by mulk's class (0: no constant operand)
         for (uint64_t &x : T.width_census) x = 0;
         // per tape word (a run of bit extractions counts once, with the width of its source)
         auto census = [&](uint32_t i, uint32_t opcode) {   // widest of the result and the slot operands (constants do not count)
@@ -1767,7 +1791,8 @@ struct Lowerer {
         // one operator as a tape word; operands that are fused producers read an accumulator
         auto word = [&](uint32_t i, uint32_t dstfield, int acc_a, int acc_b, uint32_t d[4]) {
             const uint32_t *o = &pops[(size_t)i * 4];
-            const uint32_t opcode = o[0] == 45 ? o[0] : narrow_opcode(i);
+            const MulK mk = mulk(i);
+            const uint32_t opcode = o[0] == 45 ? o[0] : (narrow_on && mk.operand != NO_SLOT) ? DOP_MULK : narrow_opcode(i);
             d[0] = opcode | (dstfield << 8);  // opcode in bits 0-7, destination in bits 8-31
             if (o[0] == 45) {
                 uint32_t n = pcalls[o[1] + 1];
@@ -1792,6 +1817,7 @@ struct Lowerer {
                 else if (k == 2 && acc_b >= 0) d[k] = OPERAND_ACC | (uint32_t)acc_b;
                 else d[k] = remap[o[k]];
             }
+            if (opcode == DOP_MULK) d[2] = mk.operand;
         };
         // post-order emission of a fused sub-tree; its value ends in accumulator `target`
         std::function<void(uint32_t, int)> emit_sub = [&](uint32_t i, int target) {
@@ -1810,7 +1836,7 @@ struct Lowerer {
             word(i, DST_ACC + (uint32_t)target, acc_a, acc_b, d);
             census(i, d[0] & 0xFFu);
             T.ops.insert(T.ops.end(), d, d + 4);
-            if (pops[(size_t)i * 4] == CW_OP_MUL) ++T.n_mul_ops;
+            if (pops[(size_t)i * 4] == CW_OP_MUL) { ++T.n_mul_ops; ++mul_census[mulk(i).cls]; }
         };
         for (size_t r = 0; r < order.size(); ++r) {
             const uint32_t i = order[r];
@@ -1855,10 +1881,15 @@ struct Lowerer {
                 T.ops.insert(T.ops.end(), d, d + 4);
             }
             prev_level = lvl;
-            if (o[0] == CW_OP_MUL) ++T.n_mul_ops;
+            if (o[0] == CW_OP_MUL) { ++T.n_mul_ops; ++mul_census[mulk(i).cls]; }
             T.level_start[lvl]++;  // work items per level (levels start at 1)
         }
         T.items.push_back((uint32_t)(T.ops.size() / 4));
+        if (const char *cenv = getenv("CW_FUSION_CENSUS"); cenv && atoi(cenv))
+            fprintf(stderr, "product census: Montgomery products by the canonical value k of their constant operand: "
+                    "no constant %llu, k < 2^32 %llu, 2^32 <= k <= 2^64 %llu, wider %llu\n",
+                    (unsigned long long)mul_census[0], (unsigned long long)mul_census[1], (unsigned long long)mul_census[2],
+                    (unsigned long long)mul_census[3]);
         // prefix sums: level_start[l-1] = first work item of level l
         {
             std::vector<uint32_t> ls(max_level + 1, 0);
@@ -2123,7 +2154,7 @@ struct BlobR {
         p += n;
     }
 };
-constexpr uint32_t BLOB_VERSION = 7;   // 7: width-classed opcodes, width census
+constexpr uint32_t BLOB_VERSION = 8;   // 7: width-classed opcodes, width census; 8: OP_MULK
 }  // namespace
 
 void serialize_tape(const Tape &t, std::vector<uint8_t> &out) {

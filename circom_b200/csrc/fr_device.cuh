@@ -657,6 +657,7 @@ enum {
     OP_ADDI = 48,     // a + b, the sum proven below 2^(qbits-1) < q: no reduction
     OP_SHRK = 49,     // a >> k, k = b[0] < qbits (a plain right shift: no "negative" amount)
     OP_SHLK = 50,     // a << k, k = b[0], the result proven below 2^(qbits-1): no mask, no wrap
+    OP_MULK = 51,     // a * k mod q, k <= 2^64 and a Barrett constant in b (fr_mul_small): MontMul(a, k R) without the CIOS
     OP_NARROW_HALF = 52,
     OP_ADDI_H = 52,   // OP_ADDI on operands and result below 2^128: 4 limbs
     OP_MULI_Q = 53,   // a * b with a, b < 2^64: 4 limb products (OP_MULSMALL takes 36)
@@ -664,6 +665,96 @@ enum {
     OP_SHRK_H = 55,   // OP_SHRK on a < 2^128
     OP_SHLK_H = 56    // OP_SHLK on a < 2^128
 };
+
+// ---- product by a small integer: a k mod q for a < q and k <= 2^64 (OP_MULK) ------------------------------------------
+// kb holds k in limbs 0-2 (k = 2^64: limbs 0-1 zero, limb 2 one) and m = mu - 2^64 in limbs 4-5, where
+// mu = floor(2^(s+65) / q) and s = qbits - 1; the lowering writes both into the operand constant (flatten.cpp).
+// Barrett reduction of t = a k <= (q - 1) 2^64: with t1 = floor(t / 2^s) < 2^65 the estimate qh = floor(t1 mu / 2^65) of
+// Q = floor(t / q) satisfies Q - 2 <= qh <= Q for every q with 2^s < q < 2^(s+1):
+//   qh <= t / q, since t1 <= t / 2^s and mu <= 2^(s+65) / q;
+//   t1 > t / 2^s - 1 and mu > 2^(s+65) / q - 1 give t1 mu / 2^65 > t/q - t / 2^(s+65) - 2^s / q > t/q - 2,
+//   since t < q 2^64 < 2^(s+65) and 2^s < q.
+// So t - qh q lies in [0, 3q) (nine limbs), and two conditional subtractions finish.  qh <= Q < 2^64.  16 + 4 + 16 limb
+// products instead of the CIOS' 136.  The limb positions below assume 224 <= s <= 255: every prime but goldilocks, which
+// never gets the opcode.
+CW_HD u64 u64_mul_hi(u64 x, u64 y) {
+#if defined(__CUDA_ARCH__)
+    return __umul64hi(x, y);
+#else
+    return (u64)(((unsigned __int128)x * y) >> 64);
+#endif
+}
+CW_HD void fr_mul_small(u32 *r, const u32 *a, const u32 *kb, const FrParams &P) {
+    u32 t[10];
+    if (kb[2]) {   // k = 2^64
+        t[0] = t[1] = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) t[j + 2] = a[j];
+    } else {
+        u64 c = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            c += (u64)a[j] * kb[0];
+            t[j] = (u32)c;
+            c >>= 32;
+        }
+        t[8] = (u32)c;
+        c = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            c += (u64)a[j] * kb[1] + t[j + 1];
+            t[j + 1] = (u32)c;
+            c >>= 32;
+        }
+        t[9] = (u32)c;
+    }
+    // t1 = t >> s = (t[7], t[8], t[9]) >> (s - 224): 64 bits and a top bit
+    const u32 sh = (P.qbits - 1u) & 31u;
+    const u64 t1 = ((((u64)t[8] << 32) | t[7]) >> sh) | ((u64)((((u64)t[9] << 32) | t[8]) >> sh) << 32);
+    const u32 t1_top = t[9] >> sh;
+    // qh = floor(t1 (2^64 + m) / 2^65) = floor((hi(t1_lo m) + t1_lo + t1_top m + t1_top 2^64) / 2)
+    const u64 m = (u64)kb[4] | ((u64)kb[5] << 32);
+    u64 x = u64_mul_hi(t1, m), y;
+    u32 cx = t1_top;
+    y = x + t1;
+    cx += y < x;
+    x = y + (t1_top ? m : 0ull);
+    cx += x < y;
+    const u64 qh = (x >> 1) | ((u64)cx << 63);
+    // r = t - qh q  mod 2^288
+    u32 p[9];
+    {
+        const u32 q0 = (u32)qh, q1 = (u32)(qh >> 32);
+        u64 c = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            c += (u64)P.q[j] * q0;
+            p[j] = (u32)c;
+            c >>= 32;
+        }
+        p[8] = (u32)c;
+        c = 0;
+#pragma unroll
+        for (int j = 0; j < 7; ++j) {
+            c += (u64)P.q[j] * q1 + p[j + 1];
+            p[j + 1] = (u32)c;
+            c >>= 32;
+        }
+        p[8] += (u32)c + P.q[7] * q1;
+    }
+    u32 br = u256_sub(r, t, p);
+    u32 r8 = t[8] - p[8] - br;
+    // two conditional subtractions of q (nine limbs; q's ninth is zero)
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        u32 d[8];
+        br = u256_sub(d, r, P.q);
+        const bool keep = r8 < br;   // r < q
+#pragma unroll
+        for (int i = 0; i < 8; ++i) r[i] = keep ? r[i] : d[i];
+        r8 = keep ? r8 : r8 - br;
+    }
+}
 
 // low 256 bits of the integer product (36 limb products instead of CIOS' 128)
 CW_HD void u256_mul_lo(u32 *r, const u32 *a, const u32 *b) {
@@ -817,6 +908,7 @@ CW_HD void fr_exec_t(u32 opcode, u32 *r, const u32 *a, const u32 *b, u32 imm, co
         case OP_ADDI: u256_add(r, a, b); break;
         case OP_SHRK: u256_shr(r, a, b[0]); break;
         case OP_SHLK: u256_shl(r, a, b[0]); break;
+        case OP_MULK: fr_mul_small(r, a, b, P); break;
         case OP_ADDI_H: u128_add(r, a, b); break;
         case OP_MULI_Q: u256_mul_narrow<2>(r, a, b); break;
         case OP_MULI_H: u256_mul_narrow<4>(r, a, b); break;

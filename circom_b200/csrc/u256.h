@@ -100,6 +100,21 @@ struct FieldParams {
     U256 to_mont(const U256 &a) const { return mont_mul(a, r2); }
     U256 from_mont(const U256 &a) const { return mont_mul(a, u256_from_u64(1)); }
     U256 mulm(const U256 &a, const U256 &b) const { return mont_mul(to_mont(a), b); }
+    // floor(2^(qbits+64) / q) - 2^64: the Barrett constant of fr_mul_small (fr_device.cuh).  The quotient lies in
+    // (2^64, 2^65) for any q strictly between two powers of two, so the 64 bits kept here determine it.
+    uint64_t barrett_mu() const {
+        U256 rem = u256_from_u64(1);
+        uint64_t quo = 0;
+        for (uint32_t i = 0; i < qbits + 64; ++i) {   // long division of 2^(qbits+64), one bit per step
+            const uint64_t carry = u256_add(rem, rem, rem);
+            quo <<= 1;
+            if (carry || !(rem < q)) {
+                u256_sub(rem, rem, q);
+                quo |= 1;
+            }
+        }
+        return quo;
+    }
 };
 
 inline FieldParams make_field(int prime_id) {

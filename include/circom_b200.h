@@ -58,7 +58,8 @@ extern "C" {
                                   of travelling through the value store: half the levels, 30 % fewer stores; pays only for large
                                   batches (measured: DESIGN.md section 7) */
 #define CW_FLAG_NO_NARROW 128u /* emit every operator at full width: no width-classed forms (plain integer ADD / MULSMALL / shifts
-                                  that read only the limbs the range analysis allows; for A/B comparisons) */
+                                  that read only the limbs the range analysis allows, products by constants k <= 2^64
+                                  without a Montgomery product; for A/B comparisons) */
 #define CW_FLAG_COMPACT (CW_FLAG_BITPLANE | CW_FLAG_REUSE) /* the compact value store: what cw_batch_* runs best on */
 #define CW_FLAG_O0 4u         /* --O0: keep every signal in the witness and every `signal = signal` constraint */
 
@@ -391,7 +392,9 @@ int cw_wtns_read(const char *path, int *prime_id, uint64_t *n_witness, uint64_t 
 int cw_r1cs_check_files(const char *r1cs_path, const char *wtns_path, int device, int64_t *first_bad);
 
 /* ---- field library, batched (parity tests of the device Fr_* equivalents, fr.hpp:28-70) ------ */
-/* r[i] = op(a[i], b[i], c[i]) for i < n on `device`; canonical in / canonical out; b, c may be NULL */
+/* r[i] = op(a[i], b[i], c[i]) for i < n on `device`; canonical in / canonical out; b, c may be NULL.  The device-only opcodes
+ * take their operands as the tape does: op 51 (MULK, 256-bit primes) is a[i] * k mod q for b[i] = k + 2^128 (mu - 2^64),
+ * k <= 2^64, mu = floor(2^(qbits+64) / q) */
 int cw_fr_batch_op(int prime_id, int op, const uint64_t *a, const uint64_t *b, const uint64_t *c,
                    uint64_t *r, size_t n, int device);
 /* Montgomery-multiplication throughput probe: n independent chains of `iters` dependent multiplications;

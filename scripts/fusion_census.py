@@ -9,6 +9,9 @@ prints
     that runs in a pass of its own (INV / POW), the operand position (SELECT's condition), the FUSE_MAX bound on a
     work item, the two-accumulator rule (a second fused operand must be a chain), and producer opcodes the pass never
     fuses (by opcode number);
+  * the lowering's census of the Montgomery products by the canonical value k = K R^-1 of their constant operand K (no
+    constant, k < 2^32, 2^32 <= k <= 2^64, wider; printed on stderr as well): the products with k <= 2^64 run as OP_MULK
+    on every prime but goldilocks, the others (conversions into Montgomery form by R^2, wide constants) stay CIOS products;
   * per witness: the stored values, the slot-operand reads, the work items, the levels and the bytes the value store
     moves (`layout_bytes`, as bench.py counts them).
 """
