@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <condition_variable>
 #include <cstring>
@@ -47,6 +48,52 @@ int fail(int code, const std::string &msg) {
         if (e_ != cudaSuccess)                                                                         \
             return fail(CW_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_));                 \
     } while (0)
+
+// Owners of device memory, pinned host memory, events and streams: the only code that releases them, so that a
+// function may return (CU) at any point without leaking what it holds.  Release on the device that is current.
+struct DevFree { void operator()(void *p) const { cudaFree(p); } };
+struct PinnedFree { void operator()(void *p) const { cudaFreeHost(p); } };
+struct EventDestroy { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct StreamDestroy { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+template <class T> using DevPtr = std::unique_ptr<T, DevFree>;
+template <class T> using PinnedPtr = std::unique_ptr<T, PinnedFree>;
+using Event = std::unique_ptr<CUevent_st, EventDestroy>;
+using Stream = std::unique_ptr<CUstream_st, StreamDestroy>;
+
+template <class T>
+int dev_alloc(DevPtr<T> &dst, size_t bytes) {
+    void *p = nullptr;
+    CU(cudaMalloc(&p, bytes));
+    dst.reset((T *)p);
+    return CW_OK;
+}
+template <class T>
+int pinned_alloc(PinnedPtr<T> &dst, size_t bytes) {
+    void *p = nullptr;
+    CU(cudaMallocHost(&p, bytes));
+    dst.reset((T *)p);
+    return CW_OK;
+}
+int make_event(Event &e, unsigned flags = cudaEventDefault) {
+    cudaEvent_t h = nullptr;
+    CU(cudaEventCreateWithFlags(&h, flags));
+    e.reset(h);
+    return CW_OK;
+}
+int make_stream(Stream &s) {
+    cudaStream_t h = nullptr;
+    CU(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking));
+    s.reset(h);
+    return CW_OK;
+}
+// `bytes` of host memory copied into a new device allocation (at least 16 bytes, so that empty tables get a pointer)
+template <class T>
+int upload(DevPtr<T> &dst, const void *src, size_t bytes) {
+    int rc = dev_alloc(dst, bytes ? bytes : 16);
+    if (rc) return rc;
+    if (bytes) CU(cudaMemcpy(dst.get(), src, bytes, cudaMemcpyHostToDevice));
+    return CW_OK;
+}
 
 FrParams make_dev_params(const FieldParams &F) {
     FrParams p;
@@ -108,35 +155,28 @@ u32 device_sms() {
 }
 
 struct DevTape {
-    uint4 *ops = nullptr;
-    u32 *items = nullptr, *level_start = nullptr, *level_info = nullptr;
+    DevPtr<uint4> ops;
+    DevPtr<u32> items, level_start, level_info;
     bool has_slow = false;
-    uint4 *heads = nullptr;  // first tape word of every work item
-    uint4 *consts = nullptr;
-    u32 *input_slot = nullptr, *fn_code = nullptr, *fn_info = nullptr, *call_tab = nullptr;
-    u32 *wloc = nullptr;  // per witness entry: where its value lives (slot id, or OPD_BIT | plane position)
+    DevPtr<uint4> heads;  // first tape word of every work item
+    DevPtr<uint4> consts;
+    DevPtr<u32> input_slot, fn_code, fn_info, call_tab;
+    DevPtr<u32> wloc;  // per witness entry: where its value lives (slot id, or OPD_BIT | plane position)
     // witness entries outside the bit plane by static size class (slot ids), for the packed device->host transfer
-    u32 *pk_bit = nullptr, *pk_u64 = nullptr, *pk_full = nullptr;
+    DevPtr<u32> pk_bit, pk_u64, pk_full;
 };
 struct DevR1cs {
-    unsigned long long *row_ptr = nullptr;
-    uint4 *terms = nullptr;  // per term {location, dictionary index, kind word, absorbed boolean row}
-    uint4 *dictM = nullptr;
-    u32 *perm = nullptr, *bool_loc = nullptr, *bool_row = nullptr;
-    u32 *perm_small = nullptr;   // rows small by shape: decided over the integers (r1cs_small.h)
-    uint2 *sgroups = nullptr, *srecs = nullptr;   // ... from a term list of their own
-    u32 *sbrow = nullptr;
+    DevPtr<unsigned long long> row_ptr;
+    DevPtr<uint4> terms;  // per term {location, dictionary index, kind word, absorbed boolean row}
+    DevPtr<uint4> dictM;
+    DevPtr<u32> perm, bool_loc, bool_row;
+    DevPtr<u32> perm_small;   // rows small by shape: decided over the integers (r1cs_small.h)
+    DevPtr<uint2> sgroups, srecs;   // ... from a term list of their own
+    DevPtr<u32> sbrow;
     u32 n_general = 0, n_bool = 0, n_small = 0;
     u32 mean_row_terms = 0;  // compiled terms per general row
     uint64_t n_terms = 0;
 };
-
-template <class T>
-int upload(T **dst, const void *src, size_t bytes) {
-    CU(cudaMalloc((void **)dst, bytes ? bytes : 16));
-    if (bytes) CU(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-    return CW_OK;
-}
 
 int env_int(const char *name, int dflt) {
     const char *s = getenv(name);
@@ -151,15 +191,13 @@ int env_int(const char *name, int dflt) {
 struct NarrowPack {
     PackLayout L;
     std::vector<uint8_t> cls;
-    u32 *pk_bit = nullptr, *pk_u64 = nullptr, *pk_full = nullptr;
-    ~NarrowPack() {
-        cudaFree(pk_bit);
-        cudaFree(pk_u64);
-        cudaFree(pk_full);
-    }
+    DevPtr<u32> pk_bit, pk_u64, pk_full;
 };
 
+static std::atomic<uint64_t> g_circuit_serial{0};
+
 struct cw_circuit {
+    const uint64_t serial = ++g_circuit_serial;   // process-wide identity of the handle (never 0): the R1CS layout key
     Tape tape;
     mutable std::mutex mu;
     mutable std::mutex narrow_mu;   // serialises the (rare) observation passes
@@ -179,7 +217,7 @@ struct cw_circuit {
 
 struct R1csKey {
     int device;
-    const cw_circuit *layout;  // nullptr: dense witness rows (location = wire id)
+    uint64_t layout;  // serial of the circuit whose value layout the CSR reads; 0: dense witness rows (location = wire id)
     bool operator<(const R1csKey &o) const { return device != o.device ? device < o.device : layout < o.layout; }
 };
 struct cw_r1cs {
@@ -187,8 +225,8 @@ struct cw_r1cs {
     FieldParams F;
     std::mutex mu;
     std::map<R1csKey, DevR1cs> dev;
-    cw_r1cs *eval_twin = nullptr;  // the same constraints compiled without boolean-row special cases (cw_r1cs_eval_batch)
-    cw_r1cs *qap_twin = nullptr;   // ... plus the rows a_{m+j} = w_j, j <= nPublic (cw_r1cs_quotient_*)
+    std::unique_ptr<cw_r1cs> eval_twin;  // the same constraints compiled without boolean-row special cases (cw_r1cs_eval_batch)
+    std::unique_ptr<cw_r1cs> qap_twin;   // ... plus the rows a_{m+j} = w_j, j <= nPublic (cw_r1cs_quotient_*)
     bool no_bool_rows = false;
 };
 
@@ -196,15 +234,15 @@ struct cw_batch {
     const cw_circuit *c = nullptr;
     int device = 0;
     u32 batch = 0, batch_padded = 0, bt_log2 = 0, threads = 256;
-    cudaStream_t stream = nullptr;
-    uint4 *slots = nullptr, *inputs_d = nullptr, *witness_d = nullptr;
-    u32 *plane = nullptr;
-    u32 *first_assert_d = nullptr;
-    int *err_d = nullptr;
-    unsigned long long *fb_d = nullptr;  // per-instance result of the R1CS check
-    u32 *r1cs_wide_d = nullptr;          // bitmap of the integer rows handed to the general kernel (launch_r1cs)
+    Stream stream;   // (declared first: released last)
+    DevPtr<uint4> slots, inputs_d, witness_d;
+    DevPtr<u32> plane;
+    DevPtr<u32> first_assert_d;
+    DevPtr<int> err_d;
+    DevPtr<unsigned long long> fb_d;  // per-instance result of the R1CS check
+    DevPtr<u32> r1cs_wide_d;          // bitmap of the integer rows handed to the general kernel (launch_r1cs)
     u32 r1cs_wide_rows = 0;
-    DevTape dt;
+    const DevTape *dt = nullptr;      // the circuit's cache entry for this device
     std::vector<uint64_t> host_inputs;  // [batch][n_inputs][4]
     std::vector<uint8_t> assigned;      // [batch][n_inputs]
     std::vector<u32> remaining;         // [batch]
@@ -214,14 +252,15 @@ struct cw_batch {
     bool dense_valid = false;  // witness_d holds the dense rows of the current run
     // packed transfer: two staging buffers (device + pinned host) so that the pack kernel and the copy of one
     // chunk overlap the host-side expansion of the previous one
-    u32 *packed_d[2] = {nullptr, nullptr}, *packed_h[2] = {nullptr, nullptr};
+    DevPtr<u32> packed_d[2];
+    PinnedPtr<u32> packed_h[2];
     size_t packed_cap = 0;  // instances per staging buffer
-    uint4 *dense_chunk_d = nullptr;
+    DevPtr<uint4> dense_chunk_d;
     size_t dense_chunk_cap = 0;
-    int *pack_flag_d = nullptr;
-    cudaEvent_t pack_ev[2] = {nullptr, nullptr};
+    DevPtr<int> pack_flag_d;  // set by the pack kernel when a value exceeds its class
+    Event pack_ev[2];
     uint64_t last_d2h_bytes = 0;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    Event ev[3];
     std::thread async_th;  // cw_batch_get_witness_async
     int async_rc = 0;
     std::string async_err;
@@ -232,8 +271,8 @@ struct cw_batch {
     }
     StoreDev store() const {
         StoreDev S;
-        S.slots = slots;
-        S.plane = plane;
+        S.slots = slots.get();
+        S.plane = plane.get();
         S.n_slots = c->tape.n_slots;
         S.n_bitwords = c->tape.n_bitwords;
         S.bt_log2 = bt_log2;
@@ -242,25 +281,37 @@ struct cw_batch {
     }
 };
 
-static int get_dev_tape(const cw_circuit *c, int device, DevTape &out) {
+// `count` dense witness rows `stride_elems` elements apart, as a value store (one instance per tile, no bit plane)
+static StoreDev dense_store(const void *rows, uint64_t stride_elems, u32 count) {
+    StoreDev S;
+    S.slots = (const uint4 *)rows;
+    S.plane = nullptr;
+    S.n_slots = (u32)stride_elems;
+    S.n_bitwords = 0;
+    S.bt_log2 = 0;
+    S.batch = count;
+    return S;
+}
+
+static int get_dev_tape(const cw_circuit *c, int device, const DevTape *&out) {
     const PackLayout &L = c->pack_layout();
     std::lock_guard<std::mutex> lk(c->mu);
     auto it = c->dev.find(device);
     if (it != c->dev.end()) {
-        out = it->second;
+        out = &it->second;
         return CW_OK;
     }
     const Tape &t = c->tape;
     DevTape d;
     int rc;
-    if ((rc = upload(&d.ops, t.ops.data(), t.ops.size() * 4))) return rc;
-    if ((rc = upload(&d.items, t.items.data(), t.items.size() * 4))) return rc;
+    if ((rc = upload(d.ops, t.ops.data(), t.ops.size() * 4))) return rc;
+    if ((rc = upload(d.items, t.items.data(), t.items.size() * 4))) return rc;
     {
         std::vector<uint32_t> heads(t.n_items() * 4);
         for (size_t k = 0; k < t.n_items(); ++k) memcpy(&heads[k * 4], &t.ops[(size_t)t.items[k] * 4], 16);
-        if ((rc = upload(&d.heads, heads.data(), heads.size() * 4))) return rc;
+        if ((rc = upload(d.heads, heads.data(), heads.size() * 4))) return rc;
     }
-    if ((rc = upload(&d.level_start, t.level_start.data(), t.level_start.size() * 4))) return rc;
+    if ((rc = upload(d.level_start, t.level_start.data(), t.level_start.size() * 4))) return rc;
     {
         // per level: how many calls close it (the lowering sorts the items of a level by opcode, CALL is the largest: the
         // kernel runs them after the other items) and whether it has INV / POW items (run in a pass of their own)
@@ -284,19 +335,18 @@ static int get_dev_tape(const cw_circuit *c, int device, DevTape &out) {
                 }
             }
         }
-        if ((rc = upload(&d.level_info, info.data(), info.size() * 4))) return rc;
+        if ((rc = upload(d.level_info, info.data(), info.size() * 4))) return rc;
     }
-    if ((rc = upload(&d.consts, t.consts.data(), t.consts.size() * 32))) return rc;
-    if ((rc = upload(&d.input_slot, t.input_slot.data(), t.input_slot.size() * 4))) return rc;
-    if ((rc = upload(&d.fn_code, t.fn_code.data(), t.fn_code.size() * 4))) return rc;
-    if ((rc = upload(&d.fn_info, t.fn_info.data(), t.fn_info.size() * 4))) return rc;
-    if ((rc = upload(&d.call_tab, t.call_tab.data(), t.call_tab.size() * 4))) return rc;
-    if ((rc = upload(&d.wloc, t.witness_slot.data(), t.witness_slot.size() * 4))) return rc;
-    if ((rc = upload(&d.pk_bit, L.bit_loc.data(), L.bit_loc.size() * 4))) return rc;
-    if ((rc = upload(&d.pk_u64, L.u64_loc.data(), L.u64_loc.size() * 4))) return rc;
-    if ((rc = upload(&d.pk_full, L.full_loc.data(), L.full_loc.size() * 4))) return rc;
-    c->dev[device] = d;
-    out = d;
+    if ((rc = upload(d.consts, t.consts.data(), t.consts.size() * 32))) return rc;
+    if ((rc = upload(d.input_slot, t.input_slot.data(), t.input_slot.size() * 4))) return rc;
+    if ((rc = upload(d.fn_code, t.fn_code.data(), t.fn_code.size() * 4))) return rc;
+    if ((rc = upload(d.fn_info, t.fn_info.data(), t.fn_info.size() * 4))) return rc;
+    if ((rc = upload(d.call_tab, t.call_tab.data(), t.call_tab.size() * 4))) return rc;
+    if ((rc = upload(d.wloc, t.witness_slot.data(), t.witness_slot.size() * 4))) return rc;
+    if ((rc = upload(d.pk_bit, L.bit_loc.data(), L.bit_loc.size() * 4))) return rc;
+    if ((rc = upload(d.pk_u64, L.u64_loc.data(), L.u64_loc.size() * 4))) return rc;
+    if ((rc = upload(d.pk_full, L.full_loc.data(), L.full_loc.size() * 4))) return rc;
+    out = &c->dev.emplace(device, std::move(d)).first->second;
     return CW_OK;
 }
 
@@ -308,14 +358,17 @@ template <int PR, bool CALLS, bool BP, int BT, bool FU>
 static void launch_tape_k(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th) {
     constexpr u32 smem = FU ? TAPE_ACC_SMEM : 0u;
     static_assert(TAPE_ACC_SMEM * CW_TAPE_LB <= 48u * 1024u, "the widest CTA stays within the default dynamic shared memory");
-    tape_exec_kernel<PR, CALLS, BP, BT, FU><<<tiles, th, smem * th, b->stream>>>(tp, b->slots, b->plane, b->bt_log2,
-                                                                                b->first_assert_d, b->err_d, b->batch);
+    tape_exec_kernel<PR, CALLS, BP, BT, FU><<<tiles, th, smem * th, b->stream.get()>>>(
+        tp, b->slots.get(), b->plane.get(), b->bt_log2, b->first_assert_d.get(), b->err_d.get(), b->batch);
+}
+static void launch_calls(int pr, const TapeDev &tp, cw_batch *b, u32 tiles, u32 th, bool bp, bool fused) {
+    launch_tape_calls(pr, tp, b->slots.get(), b->plane.get(), b->bt_log2, b->first_assert_d.get(), b->err_d.get(), b->batch,
+                      tiles, th, bp, fused, b->stream.get());
 }
 template <int PR>
 static void launch_tape(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th, bool calls, bool bp, bool fused) {
     if (calls) {  // the builds with the function machine: tape_calls.cu
-        launch_tape_calls(PR, tp, b->slots, b->plane, b->bt_log2, b->first_assert_d, b->err_d, b->batch, tiles, th, bp, fused,
-                          b->stream);
+        launch_calls(PR, tp, b, tiles, th, bp, fused);
     } else if (fused) {  // (the bit-plane build also runs tapes without a plane: they contain no plane operands)
         if (b->bt_log2 == 5) launch_tape_k<PR, false, true, 5, true>(tp, b, tiles, th);
         else launch_tape_k<PR, false, true, -1, true>(tp, b, tiles, th);
@@ -344,14 +397,13 @@ int cw_device_count(void) {
 
 int cw_circuit_load_mem(const void *data, size_t len, uint32_t flags, cw_circuit **out) {
     if (!data || !out) return fail(CW_EINVAL, "null argument");
-    cw_circuit *c = new cw_circuit();
+    auto c = std::make_unique<cw_circuit>();
     try {
         lower_circuit((const uint8_t *)data, len, flags, c->tape);
     } catch (const std::exception &e) {
-        delete c;
         return fail(CW_EFORMAT, e.what());
     }
-    *out = c;
+    *out = c.release();
     return CW_OK;
 }
 
@@ -371,22 +423,9 @@ int cw_circuit_load(const char *path, uint32_t flags, cw_circuit **out) {
 
 void cw_circuit_destroy(cw_circuit *c) {
     if (!c) return;
-    for (auto &kv : c->dev) {
-        cudaSetDevice(kv.first);
-        cudaFree(kv.second.ops);
-        cudaFree(kv.second.items);
-        cudaFree(kv.second.heads);
-        cudaFree(kv.second.level_start);
-        cudaFree(kv.second.level_info);
-        cudaFree(kv.second.consts);
-        cudaFree(kv.second.input_slot);
-        cudaFree(kv.second.fn_code);
-        cudaFree(kv.second.fn_info);
-        cudaFree(kv.second.call_tab);
-        cudaFree(kv.second.wloc);
-        cudaFree(kv.second.pk_bit);
-        cudaFree(kv.second.pk_u64);
-        cudaFree(kv.second.pk_full);
+    for (auto it = c->dev.begin(); it != c->dev.end(); it = c->dev.erase(it)) {
+        cudaSetDevice(it->first);
+        c->narrow.erase(it->first);
     }
     delete c;
 }
@@ -538,7 +577,7 @@ int cw_batch_create(const cw_circuit *c, uint32_t batch, int device, cw_batch **
     int rc = ensure_device(device);
     if (rc) return rc;
     const Tape &t = c->tape;
-    cw_batch *b = new cw_batch();
+    auto b = std::make_unique<cw_batch>();
     b->c = c;
     b->device = device;
     b->batch = batch;
@@ -578,25 +617,26 @@ int cw_batch_create(const cw_circuit *c, uint32_t batch, int device, cw_batch **
     size_t free_b = 0, total_b = 0;
     cudaMemGetInfo(&free_b, &total_b);
     size_t need = slot_bytes + plane_bytes + (size_t)batch * t.n_inputs * 32 + (64u << 20);
-    if (need > free_b) {
-        delete b;
+    if (need > free_b)
         return fail(CW_ECUDA, "batch needs " + std::to_string(need >> 20) + " MiB of device memory, " +
                                   std::to_string(free_b >> 20) + " MiB free");
-    }
-    if ((rc = get_dev_tape(c, device, b->dt))) { delete b; return rc; }
-    CU(cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking));
-    CU(cudaMalloc((void **)&b->slots, slot_bytes));
-    CU(cudaMalloc((void **)&b->plane, std::max<size_t>(plane_bytes, 16)));
-    CU(cudaMalloc((void **)&b->inputs_d, std::max<size_t>((size_t)batch * t.n_inputs * 32, 32)));
-    CU(cudaMalloc((void **)&b->first_assert_d, (size_t)batch * 4));
-    CU(cudaMalloc((void **)&b->err_d, (size_t)batch * 4));
-    CU(cudaMalloc((void **)&b->fb_d, (size_t)batch * 8));
-    for (auto &e : b->ev) CU(cudaEventCreate(&e));
-    for (auto &e : b->pack_ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    if ((rc = get_dev_tape(c, device, b->dt))) return rc;
+    if ((rc = make_stream(b->stream))) return rc;
+    if ((rc = dev_alloc(b->slots, slot_bytes))) return rc;
+    if ((rc = dev_alloc(b->plane, std::max<size_t>(plane_bytes, 16)))) return rc;
+    if ((rc = dev_alloc(b->inputs_d, std::max<size_t>((size_t)batch * t.n_inputs * 32, 32)))) return rc;
+    if ((rc = dev_alloc(b->first_assert_d, (size_t)batch * 4))) return rc;
+    if ((rc = dev_alloc(b->err_d, (size_t)batch * 4))) return rc;
+    if ((rc = dev_alloc(b->fb_d, (size_t)batch * 8))) return rc;
+    if ((rc = dev_alloc(b->pack_flag_d, 4))) return rc;
+    for (auto &e : b->ev)
+        if ((rc = make_event(e))) return rc;
+    for (auto &e : b->pack_ev)
+        if ((rc = make_event(e, cudaEventDisableTiming))) return rc;
     b->host_inputs.assign((size_t)batch * t.n_inputs * 4, 0);
     b->assigned.assign((size_t)batch * t.n_inputs, 0);
     b->remaining.assign(batch, (u32)t.n_inputs);
-    *out = b;
+    *out = b.release();
     return CW_OK;
 }
 
@@ -607,26 +647,8 @@ static void join_async(cw_batch *b) {
 
 void cw_batch_destroy(cw_batch *b) {
     if (!b) return;
-    join_async(b);
+    join_async(b);   // (the helper thread uses the members)
     cudaSetDevice(b->device);
-    cudaFree(b->slots);
-    cudaFree(b->plane);
-    cudaFree(b->inputs_d);
-    cudaFree(b->witness_d);
-    cudaFree(b->dense_chunk_d);
-    for (int k = 0; k < 2; ++k) {
-        cudaFree(b->packed_d[k]);
-        if (b->packed_h[k]) cudaFreeHost(b->packed_h[k]);
-        if (b->pack_ev[k]) cudaEventDestroy(b->pack_ev[k]);
-    }
-    cudaFree(b->pack_flag_d);
-    cudaFree(b->first_assert_d);
-    cudaFree(b->err_d);
-    cudaFree(b->fb_d);
-    cudaFree(b->r1cs_wide_d);
-    for (auto &e : b->ev)
-        if (e) cudaEventDestroy(e);
-    if (b->stream) cudaStreamDestroy(b->stream);
     delete b;
 }
 
@@ -672,8 +694,8 @@ int cw_batch_set_inputs(cw_batch *b, const uint64_t *inputs, int is_device_ptr) 
     const Tape &t = b->c->tape;
     CU(cudaSetDevice(b->device));
     size_t bytes = (size_t)b->batch * t.n_inputs * 32;
-    CU(cudaMemcpyAsync(b->inputs_d, inputs, bytes, is_device_ptr ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
-                       b->stream));
+    CU(cudaMemcpyAsync(b->inputs_d.get(), inputs, bytes, is_device_ptr ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                       b->stream.get()));
     std::fill(b->remaining.begin(), b->remaining.end(), 0u);
     b->host_inputs_dirty = false;
     b->inputs_on_device = true;
@@ -691,38 +713,39 @@ int cw_batch_run(cw_batch *b) {
                 return fail(CW_ESTATE, "Not all inputs have been set. Only " +
                                            std::to_string(t.n_inputs - b->remaining[i]) + " out of " +
                                            std::to_string(t.n_inputs) + " (instance " + std::to_string(i) + ")");
-        CU(cudaMemcpyAsync(b->inputs_d, b->host_inputs.data(), b->host_inputs.size() * 8, cudaMemcpyHostToDevice,
-                           b->stream));
+        CU(cudaMemcpyAsync(b->inputs_d.get(), b->host_inputs.data(), b->host_inputs.size() * 8, cudaMemcpyHostToDevice,
+                           b->stream.get()));
         b->host_inputs_dirty = false;
         b->inputs_on_device = true;
     }
     TapeDev tp;
-    tp.ops = b->dt.ops;
-    tp.items = b->dt.items;
-    tp.heads = b->dt.heads;
-    tp.level_start = b->dt.level_start;
-    tp.level_info = b->dt.level_info;
-    tp.has_slow = b->dt.has_slow ? 1u : 0u;
-    tp.consts = b->dt.consts;
+    tp.ops = b->dt->ops.get();
+    tp.items = b->dt->items.get();
+    tp.heads = b->dt->heads.get();
+    tp.level_start = b->dt->level_start.get();
+    tp.level_info = b->dt->level_info.get();
+    tp.has_slow = b->dt->has_slow ? 1u : 0u;
+    tp.consts = b->dt->consts.get();
     tp.n_levels = (u32)t.n_levels();
     tp.n_slots = t.n_slots;
-    tp.input_slot = b->dt.input_slot;
-    tp.fn_code = b->dt.fn_code;
-    tp.fn_info = b->dt.fn_info;
-    tp.call_tab = b->dt.call_tab;
+    tp.input_slot = b->dt->input_slot.get();
+    tp.fn_code = b->dt->fn_code.get();
+    tp.fn_info = b->dt->fn_info.get();
+    tp.call_tab = b->dt->call_tab.get();
     tp.n_inputs = (u32)t.n_inputs;
     tp.n_bitwords = t.n_bitwords;
     tp.prime = (u32)t.F.prime_id;
     // the 128-bit register machine computes over the integers and gives up when a value leaves 128 bits: right only for a
     // prime above 2^128 (every 256-bit one); goldilocks calls run on the full-width machine
     tp.vm_wide = (env_int("CW_VM_WIDE", 0) || t.F.qbits <= 128) ? 1u : 0u;
-    CU(cudaMemsetAsync(b->first_assert_d, 0xFF, (size_t)b->batch * 4, b->stream));
-    CU(cudaMemsetAsync(b->err_d, 0, (size_t)b->batch * 4, b->stream));
-    CU(cudaEventRecord(b->ev[0], b->stream));
+    CU(cudaMemsetAsync(b->first_assert_d.get(), 0xFF, (size_t)b->batch * 4, b->stream.get()));
+    CU(cudaMemsetAsync(b->err_d.get(), 0, (size_t)b->batch * 4, b->stream.get()));
+    CU(cudaEventRecord(b->ev[0].get(), b->stream.get()));
     {
         size_t total = (size_t)b->batch_padded * (t.n_inputs + 1);
         u32 grid = (u32)std::min<size_t>((total + 255) / 256, device_sms() * 8);
-        stage_inputs_kernel<<<grid, 256, 0, b->stream>>>(tp, b->inputs_d, b->slots, b->batch, b->batch_padded, b->bt_log2);
+        stage_inputs_kernel<<<grid, 256, 0, b->stream.get()>>>(tp, b->inputs_d.get(), b->slots.get(), b->batch, b->batch_padded,
+                                                               b->bt_log2);
     }
     u32 tiles = b->batch_padded >> b->bt_log2;
     if (tp.n_levels) {
@@ -734,14 +757,13 @@ int cw_batch_run(cw_batch *b) {
         else if (t.F.prime_id == 1) launch_tape<1>(tp, b, tiles, th, calls, bp, fused);
         else {  // the other 256-bit primes: one build (bit-plane capable, runtime tile size), prime index from tp.prime
             if (fused) return fail(CW_ESTATE, "CW_FLAG_FUSE is available for bn128 and bls12381");
-            if (calls) launch_tape_calls(-1, tp, b->slots, b->plane, b->bt_log2, b->first_assert_d, b->err_d, b->batch, tiles, th,
-                                         true, false, b->stream);
+            if (calls) launch_calls(-1, tp, b, tiles, th, true, false);
             else launch_tape_k<-1, false, true, -1, false>(tp, b, tiles, th);
         }
     }
-    CU(cudaEventRecord(b->ev[1], b->stream));
+    CU(cudaEventRecord(b->ev[1].get(), b->stream.get()));
     b->dense_valid = false;
-    CU(cudaEventRecord(b->ev[2], b->stream));
+    CU(cudaEventRecord(b->ev[2].get(), b->stream.get()));
     CU(cudaGetLastError());
     b->ran = true;
     return CW_OK;
@@ -750,7 +772,7 @@ int cw_batch_run(cw_batch *b) {
 int cw_batch_sync(cw_batch *b) {
     if (!b) return fail(CW_EINVAL, "null argument");
     CU(cudaSetDevice(b->device));
-    CU(cudaStreamSynchronize(b->stream));
+    CU(cudaStreamSynchronize(b->stream.get()));
     return CW_OK;
 }
 
@@ -760,9 +782,9 @@ int cw_batch_status(cw_batch *b, int32_t *status) {
     CU(cudaSetDevice(b->device));
     std::vector<u32> fa(b->batch);
     std::vector<int> er(b->batch);
-    CU(cudaMemcpyAsync(fa.data(), b->first_assert_d, (size_t)b->batch * 4, cudaMemcpyDeviceToHost, b->stream));
-    CU(cudaMemcpyAsync(er.data(), b->err_d, (size_t)b->batch * 4, cudaMemcpyDeviceToHost, b->stream));
-    CU(cudaStreamSynchronize(b->stream));
+    CU(cudaMemcpyAsync(fa.data(), b->first_assert_d.get(), (size_t)b->batch * 4, cudaMemcpyDeviceToHost, b->stream.get()));
+    CU(cudaMemcpyAsync(er.data(), b->err_d.get(), (size_t)b->batch * 4, cudaMemcpyDeviceToHost, b->stream.get()));
+    CU(cudaStreamSynchronize(b->stream.get()));
     for (u32 i = 0; i < b->batch; ++i) {
         if (er[i]) status[i] = -1;  // division by zero: the reference process aborts inside GMP
         else status[i] = fa[i] == 0xFFFFFFFFu ? 0 : (int32_t)(fa[i] + 1);
@@ -775,7 +797,7 @@ static int expand_rows(cw_batch *b, u32 first, u32 count, uint4 *dst) {
     const Tape &t = b->c->tape;
     if (count == 0) return CW_OK;
     dim3 grid((u32)std::min<size_t>((t.n_witness + 255) / 256, device_sms() * 4), std::min<u32>(count, 65535u));
-    witness_expand_kernel<<<grid, 256, 0, b->stream>>>(b->store(), b->dt.wloc, (u32)t.n_witness, first, count, dst);
+    witness_expand_kernel<<<grid, 256, 0, b->stream.get()>>>(b->store(), b->dt->wloc.get(), (u32)t.n_witness, first, count, dst);
     CU(cudaGetLastError());
     return CW_OK;
 }
@@ -784,6 +806,7 @@ static int expand_rows(cw_batch *b, u32 first, u32 count, uint4 *dst) {
 static int dense_witness(cw_batch *b) {
     if (b->dense_valid) return CW_OK;
     const Tape &t = b->c->tape;
+    int rc;
     if (!b->witness_d) {
         size_t bytes = (size_t)b->batch * t.n_witness * 32, free_b = 0, total_b = 0;
         cudaMemGetInfo(&free_b, &total_b);
@@ -791,9 +814,9 @@ static int dense_witness(cw_batch *b) {
             return fail(CW_ECUDA, "dense witness rows of the whole batch need " + std::to_string(bytes >> 20) +
                                       " MiB of device memory (" + std::to_string(free_b >> 20) +
                                       " MiB free): use cw_batch_expand_witness on a range of instances");
-        CU(cudaMalloc((void **)&b->witness_d, bytes));
+        if ((rc = dev_alloc(b->witness_d, bytes))) return rc;
     }
-    int rc = expand_rows(b, 0, b->batch, b->witness_d);
+    rc = expand_rows(b, 0, b->batch, b->witness_d.get());
     if (rc) return rc;
     b->dense_valid = true;
     return CW_OK;
@@ -830,11 +853,11 @@ static size_t pack_chunk_instances(const cw_batch *b, const PackLayout &L) {
 static int ensure_pack_buffers(cw_batch *b, const PackLayout &L) {
     if (b->packed_cap) return CW_OK;
     size_t n = pack_chunk_instances(b, L);
+    int rc;
     for (int k = 0; k < 2; ++k) {
-        CU(cudaMalloc((void **)&b->packed_d[k], n * L.words * 4));
-        CU(cudaMallocHost((void **)&b->packed_h[k], n * L.words * 4));
+        if ((rc = dev_alloc(b->packed_d[k], n * L.words * 4))) return rc;
+        if ((rc = pinned_alloc(b->packed_h[k], n * L.words * 4))) return rc;
     }
-    CU(cudaMalloc((void **)&b->pack_flag_d, 4));
     b->packed_cap = n;
     return CW_OK;
 }
@@ -844,10 +867,10 @@ static int ensure_pack_buffers(cw_batch *b, const PackLayout &L) {
 static int pack_rows(cw_batch *b, const PackLayout &L, u32 first, u32 count, u32 *dst_d, const NarrowPack *np = nullptr) {
     const size_t items = L.n_plane_words + L.n_bit_words + L.u64_loc.size() + L.full_loc.size();
     dim3 grid((u32)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, device_sms() * 4)), std::min<u32>(count, 65535u));
-    witness_pack_kernel<<<grid, 256, 0, b->stream>>>(b->store(), np ? np->pk_bit : b->dt.pk_bit, (u32)L.bit_loc.size(),
-                                                     np ? np->pk_u64 : b->dt.pk_u64, (u32)L.u64_loc.size(),
-                                                     np ? np->pk_full : b->dt.pk_full, (u32)L.full_loc.size(), dst_d, L.words,
-                                                     first, count, b->pack_flag_d);
+    witness_pack_kernel<<<grid, 256, 0, b->stream.get()>>>(
+        b->store(), (np ? np->pk_bit : b->dt->pk_bit).get(), (u32)L.bit_loc.size(), (np ? np->pk_u64 : b->dt->pk_u64).get(),
+        (u32)L.u64_loc.size(), (np ? np->pk_full : b->dt->pk_full).get(), (u32)L.full_loc.size(), dst_d, L.words, first, count,
+        b->pack_flag_d.get());
     CU(cudaGetLastError());
     return CW_OK;
 }
@@ -877,26 +900,23 @@ static int observe_classes(cw_batch *b, std::shared_ptr<NarrowPack> prev, std::s
         std::vector<u32> cls(loc.size(), 0);
         if (prev)
             for (size_t k = 0; k < loc.size(); ++k) cls[k] = prev->cls[wit[k]];
-        u32 *loc_d = nullptr, *cls_d = nullptr;
+        DevPtr<u32> loc_d, cls_d;
         int rc;
-        if ((rc = upload(&loc_d, loc.data(), loc.size() * 4))) return rc;
-        if ((rc = upload(&cls_d, cls.data(), cls.size() * 4))) { cudaFree(loc_d); return rc; }
+        if ((rc = upload(loc_d, loc.data(), loc.size() * 4))) return rc;
+        if ((rc = upload(cls_d, cls.data(), cls.size() * 4))) return rc;
         const u32 n_tiles = (b->batch + (1u << b->bt_log2) - 1) >> b->bt_log2;
         const uint64_t items = (uint64_t)loc.size() << b->bt_log2;
         dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
-        witness_observe_kernel<<<grid, 256, 0, b->stream>>>(b->store(), loc_d, (u32)loc.size(), cls_d);
-        cudaError_t e = cudaMemcpyAsync(cls.data(), cls_d, cls.size() * 4, cudaMemcpyDeviceToHost, b->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
-        cudaFree(loc_d);
-        cudaFree(cls_d);
-        if (e != cudaSuccess) return fail(CW_ECUDA, cudaGetErrorString(e));
+        witness_observe_kernel<<<grid, 256, 0, b->stream.get()>>>(b->store(), loc_d.get(), (u32)loc.size(), cls_d.get());
+        CU(cudaMemcpyAsync(cls.data(), cls_d.get(), cls.size() * 4, cudaMemcpyDeviceToHost, b->stream.get()));
+        CU(cudaStreamSynchronize(b->stream.get()));
         for (size_t k = 0; k < loc.size(); ++k) np->cls[wit[k]] = (uint8_t)std::min<u32>(cls[k], t.wit_class[wit[k]]);
     }
     build_pack_layout(t, np->L, np->cls.data());
     int rc;
-    if ((rc = upload(&np->pk_bit, np->L.bit_loc.data(), np->L.bit_loc.size() * 4))) return rc;
-    if ((rc = upload(&np->pk_u64, np->L.u64_loc.data(), np->L.u64_loc.size() * 4))) return rc;
-    if ((rc = upload(&np->pk_full, np->L.full_loc.data(), np->L.full_loc.size() * 4))) return rc;
+    if ((rc = upload(np->pk_bit, np->L.bit_loc.data(), np->L.bit_loc.size() * 4))) return rc;
+    if ((rc = upload(np->pk_u64, np->L.u64_loc.data(), np->L.u64_loc.size() * 4))) return rc;
+    if ((rc = upload(np->pk_full, np->L.full_loc.data(), np->L.full_loc.size() * 4))) return rc;
     {
         std::lock_guard<std::mutex> lk(c->mu);
         c->narrow[b->device] = np;
@@ -951,30 +971,31 @@ static int get_witness_packed_with(cw_batch *b, uint64_t *out, const PackLayout 
     const Tape &t = b->c->tape;
     int rc = ensure_pack_buffers(b, Lstatic);
     if (rc) return rc;
-    CU(cudaMemsetAsync(b->pack_flag_d, 0, 4, b->stream));
+    CU(cudaMemsetAsync(b->pack_flag_d.get(), 0, 4, b->stream.get()));
     const size_t W = t.n_witness, cap = b->packed_cap;
     const size_t n_chunks = (b->batch + cap - 1) / cap;
     Pool &pool = Pool::get(device_numa_node(b->device));
     auto expand_chunk = [&](size_t k) {
         const size_t first = k * cap, cnt = std::min(cap, b->batch - first);
-        const uint32_t *src = b->packed_h[k & 1];
+        const uint32_t *src = b->packed_h[k & 1].get();
         // item key = instance index: the rows of instance i of `out` are always written by the same (pinned) worker
         pool.parallel_for(cnt, first, [&](size_t i) { expand_record(L, src + i * L.words, out + (first + i) * W * 4); });
     };
     for (size_t k = 0; k < n_chunks; ++k) {
         const size_t first = k * cap, cnt = std::min(cap, b->batch - first);
         // staging buffer k & 1 was consumed by the expansion of chunk k - 2, which finished before chunk k - 1 was waited for
-        if ((rc = pack_rows(b, L, (u32)first, (u32)cnt, b->packed_d[k & 1], np))) return rc;
-        CU(cudaMemcpyAsync(b->packed_h[k & 1], b->packed_d[k & 1], cnt * L.words * 4, cudaMemcpyDeviceToHost, b->stream));
-        CU(cudaEventRecord(b->pack_ev[k & 1], b->stream));
+        if ((rc = pack_rows(b, L, (u32)first, (u32)cnt, b->packed_d[k & 1].get(), np))) return rc;
+        CU(cudaMemcpyAsync(b->packed_h[k & 1].get(), b->packed_d[k & 1].get(), cnt * L.words * 4, cudaMemcpyDeviceToHost,
+                           b->stream.get()));
+        CU(cudaEventRecord(b->pack_ev[k & 1].get(), b->stream.get()));
         if (k > 0) {
-            CU(cudaEventSynchronize(b->pack_ev[(k - 1) & 1]));
+            CU(cudaEventSynchronize(b->pack_ev[(k - 1) & 1].get()));
             expand_chunk(k - 1);
         }
     }
     int flag = 0;
-    CU(cudaMemcpyAsync(&flag, b->pack_flag_d, 4, cudaMemcpyDeviceToHost, b->stream));
-    CU(cudaStreamSynchronize(b->stream));
+    CU(cudaMemcpyAsync(&flag, b->pack_flag_d.get(), 4, cudaMemcpyDeviceToHost, b->stream.get()));
+    CU(cudaStreamSynchronize(b->stream.get()));
     if (flag) {   // a value exceeded its class: the rows written so far are overwritten by the next attempt
         *flagged = true;
         return CW_OK;
@@ -993,23 +1014,24 @@ static int get_witness_impl(cw_batch *b, uint64_t *out) {
     if (done) return CW_OK;
     b->last_d2h_bytes = (uint64_t)b->batch * t.n_witness * 32;
     if (b->identity_layout()) {  // rows are read in place: pitched device-to-host copy
-        CU(cudaMemcpy2DAsync(out, (size_t)t.n_witness * 32, b->slots, (size_t)t.n_slots * 32, (size_t)t.n_witness * 32,
-                             b->batch, cudaMemcpyDeviceToHost, b->stream));
-        CU(cudaStreamSynchronize(b->stream));
+        CU(cudaMemcpy2DAsync(out, (size_t)t.n_witness * 32, b->slots.get(), (size_t)t.n_slots * 32, (size_t)t.n_witness * 32,
+                             b->batch, cudaMemcpyDeviceToHost, b->stream.get()));
+        CU(cudaStreamSynchronize(b->stream.get()));
         return CW_OK;
     }
     // dense rows, a bounded number of instances at a time
     const size_t row = (size_t)t.n_witness * 32;
     if (!b->dense_chunk_d) {
         size_t n = std::max<size_t>(1, std::min<size_t>(b->batch, ((size_t)512 << 20) / row));
-        CU(cudaMalloc((void **)&b->dense_chunk_d, n * row));
+        if ((rc = dev_alloc(b->dense_chunk_d, n * row))) return rc;
         b->dense_chunk_cap = n;
     }
     for (size_t first = 0; first < b->batch; first += b->dense_chunk_cap) {
         const size_t cnt = std::min(b->dense_chunk_cap, b->batch - first);
-        if ((rc = expand_rows(b, (u32)first, (u32)cnt, b->dense_chunk_d))) return rc;
-        CU(cudaMemcpyAsync((uint8_t *)out + first * row, b->dense_chunk_d, cnt * row, cudaMemcpyDeviceToHost, b->stream));
-        CU(cudaStreamSynchronize(b->stream));
+        if ((rc = expand_rows(b, (u32)first, (u32)cnt, b->dense_chunk_d.get()))) return rc;
+        CU(cudaMemcpyAsync((uint8_t *)out + first * row, b->dense_chunk_d.get(), cnt * row, cudaMemcpyDeviceToHost,
+                           b->stream.get()));
+        CU(cudaStreamSynchronize(b->stream.get()));
     }
     return CW_OK;
 }
@@ -1055,15 +1077,16 @@ int cw_batch_get_witness_packed(cw_batch *b, uint32_t *out_words) {
     const PackLayout &L = b->c->pack_layout();
     int rc = ensure_pack_buffers(b, L);
     if (rc) return rc;
-    CU(cudaMemsetAsync(b->pack_flag_d, 0, 4, b->stream));
+    CU(cudaMemsetAsync(b->pack_flag_d.get(), 0, 4, b->stream.get()));
     for (size_t first = 0; first < b->batch; first += b->packed_cap) {
         const size_t cnt = std::min(b->packed_cap, b->batch - first);
-        if ((rc = pack_rows(b, L, (u32)first, (u32)cnt, b->packed_d[0]))) return rc;
-        CU(cudaMemcpyAsync(out_words + first * L.words, b->packed_d[0], cnt * L.words * 4, cudaMemcpyDeviceToHost, b->stream));
-        CU(cudaStreamSynchronize(b->stream));
+        if ((rc = pack_rows(b, L, (u32)first, (u32)cnt, b->packed_d[0].get()))) return rc;
+        CU(cudaMemcpyAsync(out_words + first * L.words, b->packed_d[0].get(), cnt * L.words * 4, cudaMemcpyDeviceToHost,
+                           b->stream.get()));
+        CU(cudaStreamSynchronize(b->stream.get()));
     }
     int flag = 0;
-    CU(cudaMemcpy(&flag, b->pack_flag_d, 4, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&flag, b->pack_flag_d.get(), 4, cudaMemcpyDeviceToHost));
     if (flag) return fail(CW_ESTATE, "a witness value exceeds the width the lowering proved for it");
     return CW_OK;
 }
@@ -1074,7 +1097,7 @@ int cw_batch_witness_device(cw_batch *b, const uint64_t **dptr) {
     CU(cudaSetDevice(b->device));
     int rc = dense_witness(b);
     if (rc) return rc;
-    *dptr = (const uint64_t *)b->witness_d;
+    *dptr = (const uint64_t *)b->witness_d.get();
     return CW_OK;
 }
 
@@ -1082,7 +1105,7 @@ int cw_batch_witness_strided(cw_batch *b, const uint64_t **dptr, uint64_t *strid
     if (!b || !dptr || !stride_elems) return fail(CW_EINVAL, "null argument");
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     if (b->identity_layout()) {
-        *dptr = (const uint64_t *)b->slots;
+        *dptr = (const uint64_t *)b->slots.get();
         *stride_elems = b->c->tape.n_slots;
         return CW_OK;
     }
@@ -1091,14 +1114,28 @@ int cw_batch_witness_strided(cw_batch *b, const uint64_t **dptr, uint64_t *strid
     return rc;
 }
 
-void *cw_batch_stream(cw_batch *b) { return b ? (void *)b->stream : nullptr; }
+void *cw_batch_stream(cw_batch *b) { return b ? (void *)b->stream.get() : nullptr; }
 
 int cw_batch_last_ms(cw_batch *b, float *exec_ms, float *gather_ms) {
     if (!b || !b->ran) return fail(CW_ESTATE, "batch has not been run");
     CU(cudaSetDevice(b->device));
-    CU(cudaEventSynchronize(b->ev[2]));
-    if (exec_ms) CU(cudaEventElapsedTime(exec_ms, b->ev[0], b->ev[1]));
+    CU(cudaEventSynchronize(b->ev[2].get()));
+    if (exec_ms) CU(cudaEventElapsedTime(exec_ms, b->ev[0].get(), b->ev[1].get()));
     if (gather_ms) *gather_ms = 0.f;  // no gather pass: witness entries are written in place by the tape
+    return CW_OK;
+}
+
+// the dense row of one instance, in host memory (for the .wtns writer and the log)
+static int fetch_row(cw_batch *b, u32 inst, std::vector<uint64_t> &w) {
+    const Tape &t = b->c->tape;
+    CU(cudaSetDevice(b->device));
+    w.resize((size_t)t.n_witness * 4);
+    DevPtr<uint4> row;
+    int rc;
+    if ((rc = dev_alloc(row, (size_t)t.n_witness * 32))) return rc;
+    if ((rc = expand_rows(b, inst, 1, row.get()))) return rc;
+    CU(cudaMemcpyAsync(w.data(), row.get(), (size_t)t.n_witness * 32, cudaMemcpyDeviceToHost, b->stream.get()));
+    CU(cudaStreamSynchronize(b->stream.get()));
     return CW_OK;
 }
 
@@ -1111,17 +1148,8 @@ int cw_batch_wtns_bytes(cw_batch *b, uint32_t inst, uint8_t *out, size_t cap, si
     if (len) *len = need;
     if (!out) return CW_OK;
     if (cap < need) return fail(CW_EINVAL, "buffer too small");
-    CU(cudaSetDevice(b->device));
-    std::vector<uint64_t> w((size_t)t.n_witness * 4);
-    uint4 *row = nullptr;
-    CU(cudaMalloc((void **)&row, (size_t)t.n_witness * 32));
-    int rc = expand_rows(b, inst, 1, row);
-    if (!rc) {
-        cudaError_t e = cudaMemcpyAsync(w.data(), row, (size_t)t.n_witness * 32, cudaMemcpyDeviceToHost, b->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
-        if (e != cudaSuccess) rc = fail(CW_ECUDA, cudaGetErrorString(e));
-    }
-    cudaFree(row);
+    std::vector<uint64_t> w;
+    int rc = fetch_row(b, inst, w);
     if (rc) return rc;
     std::vector<uint8_t> bytes = wtns_bytes(t.F, w.data(), t.n_witness);
     memcpy(out, bytes.data(), need);
@@ -1210,15 +1238,14 @@ int cw_r1cs_from_circuit(const cw_circuit *c, cw_r1cs **out) {
 }
 int cw_r1cs_load(const char *path, cw_r1cs **out) {
     if (!path || !out) return fail(CW_EINVAL, "null argument");
-    cw_r1cs *r = new cw_r1cs();
+    auto r = std::make_unique<cw_r1cs>();
     try {
         read_r1cs(path, r->data);
     } catch (const std::exception &e) {
-        delete r;
         return fail(CW_EFORMAT, e.what());
     }
     r->F = make_field(r->data.prime_id);
-    *out = r;
+    *out = r.release();
     return CW_OK;
 }
 int cw_r1cs_write(const cw_r1cs *r, const char *path, uint32_t n_pub_out, uint32_t n_pub_in, uint32_t n_prv_in) {
@@ -1244,26 +1271,14 @@ int cw_r1cs_info(const cw_r1cs *r, uint64_t *n_wires, uint64_t *n_constraints, u
 }
 void cw_r1cs_destroy(cw_r1cs *r) {
     if (!r) return;
-    if (r->eval_twin) cw_r1cs_destroy(r->eval_twin);
-    if (r->qap_twin) cw_r1cs_destroy(r->qap_twin);
-    for (auto &kv : r->dev) {
-        cudaSetDevice(kv.first.device);
-        cudaFree(kv.second.row_ptr);
-        cudaFree(kv.second.terms);
-        cudaFree(kv.second.dictM);
-        cudaFree(kv.second.perm);
-        cudaFree(kv.second.perm_small);
-        cudaFree(kv.second.sgroups);
-        cudaFree(kv.second.srecs);
-        cudaFree(kv.second.sbrow);
-        cudaFree(kv.second.bool_loc);
-        cudaFree(kv.second.bool_row);
-    }
+    cw_r1cs_destroy(r->eval_twin.release());
+    cw_r1cs_destroy(r->qap_twin.release());
+    for (auto it = r->dev.begin(); it != r->dev.end(); it = r->dev.erase(it)) cudaSetDevice(it->first.device);
     delete r;
 }
 
 // The CSR compiled for one value layout (r1cs_compile.cpp), uploaded.
-static int compile_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, DevR1cs &d) {
+static int compile_r1cs(cw_r1cs *r, const cw_circuit *layout, DevR1cs &d) {
     R1csCompiled h;
     try {
         compile_r1cs_host(r->data, r->F, layout ? &layout->tape : nullptr, r->no_bool_rows,
@@ -1278,32 +1293,32 @@ static int compile_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, DevR1c
     d.n_bool = (u32)h.bool_loc.size();
     d.n_terms = h.n_terms;
     d.mean_row_terms = h.mean_row_terms;
-    if ((rc = upload(&d.terms, h.terms.data(), h.terms.size() * sizeof(uint4)))) return rc;
-    if ((rc = upload(&d.bool_loc, h.bool_loc.data(), h.bool_loc.size() * 4))) return rc;
-    if ((rc = upload(&d.bool_row, h.bool_row.data(), h.bool_row.size() * 4))) return rc;
-    if ((rc = upload(&d.row_ptr, h.row_ptr.data(), h.row_ptr.size() * 8))) return rc;
-    if ((rc = upload(&d.dictM, h.dictM.data(), h.dictM.size() * 32))) return rc;
-    if ((rc = upload(&d.perm, h.perm.data(), h.perm.size() * 4))) return rc;
-    if ((rc = upload(&d.perm_small, h.perm_small.data(), h.perm_small.size() * 4))) return rc;
+    if ((rc = upload(d.terms, h.terms.data(), h.terms.size() * sizeof(uint4)))) return rc;
+    if ((rc = upload(d.bool_loc, h.bool_loc.data(), h.bool_loc.size() * 4))) return rc;
+    if ((rc = upload(d.bool_row, h.bool_row.data(), h.bool_row.size() * 4))) return rc;
+    if ((rc = upload(d.row_ptr, h.row_ptr.data(), h.row_ptr.size() * 8))) return rc;
+    if ((rc = upload(d.dictM, h.dictM.data(), h.dictM.size() * 32))) return rc;
+    if ((rc = upload(d.perm, h.perm.data(), h.perm.size() * 4))) return rc;
+    if ((rc = upload(d.perm_small, h.perm_small.data(), h.perm_small.size() * 4))) return rc;
     static_assert(sizeof(R1csSmallRec) == sizeof(uint2), "integer-row records are read as uint2");
-    if ((rc = upload(&d.sgroups, h.sgroups.data(), h.sgroups.size() * 4))) return rc;
-    if ((rc = upload(&d.srecs, h.srecs.data(), h.srecs.size() * sizeof(uint2)))) return rc;
-    if ((rc = upload(&d.sbrow, h.sbrow.data(), h.sbrow.size() * 4))) return rc;
-    (void)device;
+    if ((rc = upload(d.sgroups, h.sgroups.data(), h.sgroups.size() * 4))) return rc;
+    if ((rc = upload(d.srecs, h.srecs.data(), h.srecs.size() * sizeof(uint2)))) return rc;
+    if ((rc = upload(d.sbrow, h.sbrow.data(), h.sbrow.size() * 4))) return rc;
     return CW_OK;
 }
 
-static int get_dev_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, DevR1cs &d) {
+// the CSR of r for the value layout of `layout` (nullptr: dense rows) on `device`, compiled on first use
+static int get_dev_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, const DevR1cs *&out) {
     std::lock_guard<std::mutex> lk(r->mu);
-    R1csKey key{device, layout};
+    R1csKey key{device, layout ? layout->serial : 0};
     auto it = r->dev.find(key);
-    if (it != r->dev.end()) {
-        d = it->second;
-        return CW_OK;
+    if (it == r->dev.end()) {
+        DevR1cs d;
+        int rc = compile_r1cs(r, layout, d);
+        if (rc) return rc;
+        it = r->dev.emplace(key, std::move(d)).first;
     }
-    int rc = compile_r1cs(r, device, layout, d);
-    if (rc) return rc;
-    r->dev[key] = d;
+    out = &it->second;
     return CW_OK;
 }
 
@@ -1320,10 +1335,10 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
                        const R1csOut *eval, u32 *wide) {
     const R1csData &R = r->data;
     R1csDev rd;
-    rd.row_ptr = d.row_ptr;
-    rd.terms = d.terms;
-    rd.dictM = d.dictM;
-    rd.perm = d.perm;
+    rd.row_ptr = d.row_ptr.get();
+    rd.terms = d.terms.get();
+    rd.dictM = d.dictM.get();
+    rd.perm = d.perm.get();
     rd.n_rows = d.n_general;
     rd.prime = (u32)R.prime_id;
     const u32 bt_mask = (1u << S.bt_log2) - 1u;
@@ -1356,14 +1371,14 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
         // through the general kernel afterwards
         if (!wide || eval) return fail(CW_ESTATE, "integer rows need their scratch bitmap");
         CU(cudaMemsetAsync(wide, 0, (((size_t)d.n_small + 31) / 32 + 1) * 4, stream));
-        rd.perm = d.perm_small;
+        rd.perm = d.perm_small.get();
         rd.n_rows = d.n_small;
         const uint64_t items = (uint64_t)d.n_small << S.bt_log2;
         dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
         R1csSmallDev sg;
-        sg.groups = d.sgroups;
-        sg.recs = d.srecs;
-        sg.brow = d.sbrow;
+        sg.groups = d.sgroups.get();
+        sg.recs = d.srecs.get();
+        sg.brow = d.sbrow.get();
         if (S.bt_log2 == 0) r1cs_small_kernel<true><<<grid, 256, 0, stream>>>(rd, sg, S, fb_d, wide);
         else r1cs_small_kernel<false><<<grid, 256, 0, stream>>>(rd, sg, S, fb_d, wide);
         EvalOut eo;
@@ -1374,7 +1389,7 @@ static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStre
     if (d.n_bool && !eval) {
         const uint64_t items = (uint64_t)d.n_bool << S.bt_log2;
         dim3 bgrid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
-        r1cs_bool_kernel<<<bgrid, 256, 0, stream>>>(d.bool_loc, d.bool_row, d.n_bool, S, fb_d);
+        r1cs_bool_kernel<<<bgrid, 256, 0, stream>>>(d.bool_loc.get(), d.bool_row.get(), d.n_bool, S, fb_d);
     }
     CU(cudaGetLastError());
     return CW_OK;
@@ -1386,6 +1401,27 @@ int cw_r1cs_check(cw_r1cs *r, const uint64_t *witness, int is_device_ptr, uint32
     return cw_r1cs_check_strided(r, witness, r->data.n_wires, is_device_ptr, batch, device, first_bad, kernel_ms);
 }
 
+// the check of store S on `stream` (launch_r1cs), timed by events around the kernels; first_bad[i] = the first violated
+// row of instance i, or -1
+static int check_store(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStream_t stream, unsigned long long *fb_d,
+                       u32 *wide, int64_t *first_bad, float *kernel_ms) {
+    Event e0, e1;
+    int rc;
+    if ((rc = make_event(e0)) || (rc = make_event(e1))) return rc;
+    CU(cudaMemsetAsync(fb_d, 0xFF, (size_t)S.batch * 8, stream));
+    CU(cudaEventRecord(e0.get(), stream));
+    if ((rc = launch_r1cs(r, d, S, stream, fb_d, nullptr, wide))) return rc;
+    CU(cudaEventRecord(e1.get(), stream));
+    std::vector<unsigned long long> fb(S.batch);
+    CU(cudaMemcpyAsync(fb.data(), fb_d, (size_t)S.batch * 8, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    float ms = 0;
+    CU(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
+    if (kernel_ms) *kernel_ms = ms;
+    for (u32 i = 0; i < S.batch; ++i) first_bad[i] = fb[i] == ~0ull ? -1 : (int64_t)fb[i];
+    return CW_OK;
+}
+
 // dense witness rows handed in by the caller (host or device memory)
 int cw_r1cs_check_strided(cw_r1cs *r, const uint64_t *witness, uint64_t stride_elems, int is_device_ptr, uint32_t batch,
                           int device, int64_t *first_bad, float *kernel_ms) {
@@ -1395,50 +1431,23 @@ int cw_r1cs_check_strided(cw_r1cs *r, const uint64_t *witness, uint64_t stride_e
         return fail(CW_EINVAL, "device witness pointer must be 32-byte aligned (elements are read with 256-bit loads)");
     int rc = ensure_device(device);
     if (rc) return rc;
-    DevR1cs d;
+    const DevR1cs *d;
     if ((rc = get_dev_r1cs(r, device, nullptr, d))) return rc;
     const R1csData &R = r->data;
-    const uint4 *w_d = (const uint4 *)witness;
-    uint4 *tmp = nullptr;
+    const void *w_d = witness;
+    DevPtr<uint4> tmp;
     if (!is_device_ptr) {
-        CU(cudaMalloc((void **)&tmp, (size_t)batch * R.n_wires * 32));
-        CU(cudaMemcpy2D(tmp, (size_t)R.n_wires * 32, witness, (size_t)stride_elems * 32, (size_t)R.n_wires * 32, batch,
+        if ((rc = dev_alloc(tmp, (size_t)batch * R.n_wires * 32))) return rc;
+        CU(cudaMemcpy2D(tmp.get(), (size_t)R.n_wires * 32, witness, (size_t)stride_elems * 32, (size_t)R.n_wires * 32, batch,
                         cudaMemcpyHostToDevice));
-        w_d = tmp;
+        w_d = tmp.get();
         stride_elems = R.n_wires;
     }
-    unsigned long long *fb_d = nullptr;
-    CU(cudaMalloc((void **)&fb_d, (size_t)batch * 8));
-    CU(cudaMemset(fb_d, 0xFF, (size_t)batch * 8));
-    StoreDev S;
-    S.slots = w_d;
-    S.plane = nullptr;
-    S.n_slots = (u32)stride_elems;
-    S.n_bitwords = 0;
-    S.bt_log2 = 0;
-    S.batch = batch;
-    u32 *wide_d = nullptr;
-    if (d.n_small) CU(cudaMalloc((void **)&wide_d, (((size_t)d.n_small + 31) / 32 + 1) * 4));
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    CU(cudaEventRecord(e0));
-    rc = launch_r1cs(r, d, S, nullptr, fb_d, nullptr, wide_d);
-    CU(cudaEventRecord(e1));
-    if (!rc) {
-        std::vector<unsigned long long> fb(batch);
-        CU(cudaMemcpy(fb.data(), fb_d, (size_t)batch * 8, cudaMemcpyDeviceToHost));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, e0, e1));
-        if (kernel_ms) *kernel_ms = ms;
-        for (u32 i = 0; i < batch; ++i) first_bad[i] = fb[i] == ~0ull ? -1 : (int64_t)fb[i];
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(fb_d);
-    if (wide_d) cudaFree(wide_d);
-    if (tmp) cudaFree(tmp);
-    return rc;
+    DevPtr<unsigned long long> fb_d;
+    DevPtr<u32> wide_d;
+    if ((rc = dev_alloc(fb_d, (size_t)batch * 8))) return rc;
+    if (d->n_small && (rc = dev_alloc(wide_d, (((size_t)d->n_small + 31) / 32 + 1) * 4))) return rc;
+    return check_store(r, *d, dense_store(w_d, stride_elems, batch), nullptr, fb_d.get(), wide_d.get(), first_bad, kernel_ms);
 }
 
 // The witnesses of a batch where the tape left them (resident slots + bit plane, any tile layout): no dense rows
@@ -1449,36 +1458,17 @@ int cw_r1cs_check_batch(cw_r1cs *r, cw_batch *b, int64_t *first_bad, float *kern
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     if (r->data.prime_id != b->c->tape.F.prime_id) return fail(CW_EINVAL, "the R1CS and the batch use different primes");
     CU(cudaSetDevice(b->device));
-    DevR1cs d;
+    const DevR1cs *d;
     int rc = get_dev_r1cs(r, b->device, b->c, d);
     if (rc) return rc;
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    CU(cudaMemsetAsync(b->fb_d, 0xFF, (size_t)b->batch * 8, b->stream));
-    if (d.n_small > b->r1cs_wide_rows) {   // scratch of the integer rows: grows with the largest R1CS this batch has checked
-        CU(cudaStreamSynchronize(b->stream));
-        cudaFree(b->r1cs_wide_d);
-        b->r1cs_wide_d = nullptr;
+    if (d->n_small > b->r1cs_wide_rows) {   // scratch of the integer rows: grows with the largest R1CS this batch has checked
+        CU(cudaStreamSynchronize(b->stream.get()));
+        b->r1cs_wide_d.reset();
         b->r1cs_wide_rows = 0;
-        CU(cudaMalloc((void **)&b->r1cs_wide_d, (((size_t)d.n_small + 31) / 32 + 1) * 4));
-        b->r1cs_wide_rows = d.n_small;
+        if ((rc = dev_alloc(b->r1cs_wide_d, (((size_t)d->n_small + 31) / 32 + 1) * 4))) return rc;
+        b->r1cs_wide_rows = d->n_small;
     }
-    CU(cudaEventRecord(e0, b->stream));
-    rc = launch_r1cs(r, d, b->store(), b->stream, b->fb_d, nullptr, b->r1cs_wide_d);
-    CU(cudaEventRecord(e1, b->stream));
-    if (!rc) {
-        std::vector<unsigned long long> fb(b->batch);
-        CU(cudaMemcpyAsync(fb.data(), b->fb_d, (size_t)b->batch * 8, cudaMemcpyDeviceToHost, b->stream));
-        CU(cudaStreamSynchronize(b->stream));
-        float ms = 0;
-        CU(cudaEventElapsedTime(&ms, e0, e1));
-        if (kernel_ms) *kernel_ms = ms;
-        for (u32 i = 0; i < b->batch; ++i) first_bad[i] = fb[i] == ~0ull ? -1 : (int64_t)fb[i];
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    return rc;
+    return check_store(r, *d, b->store(), b->stream.get(), b->fb_d.get(), b->r1cs_wide_d.get(), first_bad, kernel_ms);
 }
 
 static int copy_text(const std::string &msg, char *buf, size_t cap, size_t *len) {
@@ -1501,17 +1491,8 @@ int cw_batch_log(cw_batch *b, uint32_t inst, char *buf, size_t cap, size_t *len)
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     const Tape &t = b->c->tape;
     if (t.log_args.empty()) return copy_text(std::string(), buf, cap, len);
-    CU(cudaSetDevice(b->device));
-    std::vector<uint64_t> w((size_t)t.n_witness * 4);
-    uint4 *row = nullptr;
-    CU(cudaMalloc((void **)&row, (size_t)t.n_witness * 32));
-    int rc = expand_rows(b, inst, 1, row);       // (the dense row of one instance, as the .wtns writer fetches it)
-    if (!rc) {
-        cudaError_t e = cudaMemcpyAsync(w.data(), row, (size_t)t.n_witness * 32, cudaMemcpyDeviceToHost, b->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(b->stream);
-        if (e != cudaSuccess) rc = fail(CW_ECUDA, cudaGetErrorString(e));
-    }
-    cudaFree(row);
+    std::vector<uint64_t> w;
+    int rc = fetch_row(b, inst, w);
     if (rc) return rc;
     return copy_text(format_log(t, w.data()), buf, cap, len);
 }
@@ -1547,13 +1528,7 @@ int cw_circuit_assert_info(const cw_circuit *c, uint32_t assert_no, char *buf, s
         }
         msg += ". Followed trace of components: " + trace;
     }
-    if (len) *len = msg.size();
-    if (buf && cap) {
-        const size_t n = std::min(msg.size(), cap - 1);
-        memcpy(buf, msg.data(), n);
-        buf[n] = 0;
-    }
-    return CW_OK;
+    return copy_text(msg, buf, cap, len);
 }
 
 int cw_r1cs_compiled_info(cw_r1cs *r, cw_batch *b, int device, uint64_t info[4]) {
@@ -1561,13 +1536,44 @@ int cw_r1cs_compiled_info(cw_r1cs *r, cw_batch *b, int device, uint64_t info[4])
     int rc = b ? CW_OK : ensure_device(device);
     if (rc) return rc;
     if (b) CU(cudaSetDevice(b->device));
-    DevR1cs d;
+    const DevR1cs *d;
     if ((rc = get_dev_r1cs(r, b ? b->device : device, b ? b->c : nullptr, d))) return rc;
-    info[0] = d.n_general;
-    info[1] = d.n_small;
-    info[2] = d.n_bool;
-    info[3] = d.n_terms;
+    info[0] = d->n_general;
+    info[1] = d->n_small;
+    info[2] = d->n_bool;
+    info[3] = d->n_terms;
     return CW_OK;
+}
+
+// r's constraints compiled with every row general (no boolean-row special cases): the twin of cw_r1cs_eval_batch, or
+// with `qap` that of the quotient, which appends the rows a_{m+j} = 1 * w_j (j <= n_public)
+static cw_r1cs *general_twin(cw_r1cs *r, bool qap, u32 n_public = 0) {
+    std::lock_guard<std::mutex> lk(r->mu);
+    std::unique_ptr<cw_r1cs> &twin = qap ? r->qap_twin : r->eval_twin;
+    if (twin) return twin.get();
+    auto t = std::make_unique<cw_r1cs>();
+    t->data = r->data;
+    t->F = r->F;
+    t->no_bool_rows = true;
+    if (qap) {
+        R1csData &D = t->data;
+        D.has_custom_gates = false;
+        D.gates_used.clear();
+        D.gates_applied.clear();
+        const U256 one = u256_from_u64(1);
+        u32 one_idx = (u32)D.dict.size();
+        for (size_t i = 0; i < D.dict.size(); ++i)
+            if (D.dict[i] == one) { one_idx = (u32)i; break; }
+        if (one_idx == D.dict.size()) D.dict.push_back(one);
+        for (u32 j = 0; j <= n_public; ++j) {   // row_ptr[3 m] (the end of the last row) is the start of the new row's A block
+            D.col.push_back(j);
+            D.coef.push_back(one_idx);
+            for (int k = 0; k < 3; ++k) D.row_ptr.push_back(D.col.size());
+        }
+        D.n_constraints += n_public + 1;
+    }
+    twin = std::move(t);
+    return twin.get();
 }
 
 // A.w, B.w, C.w of every constraint for instances [first, first + count) of a batch, left in device memory for a
@@ -1582,19 +1588,8 @@ int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, 
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     if (r->data.prime_id != b->c->tape.F.prime_id) return fail(CW_EINVAL, "the R1CS and the batch use different primes");
     CU(cudaSetDevice(b->device));
-    // all rows through the general path: a layout key of its own (no boolean-row special cases)
-    cw_r1cs *all = nullptr;
-    {
-        std::lock_guard<std::mutex> lk(r->mu);
-        if (!r->eval_twin) {
-            r->eval_twin = new cw_r1cs();
-            r->eval_twin->data = r->data;
-            r->eval_twin->F = r->F;
-            r->eval_twin->no_bool_rows = true;
-        }
-        all = r->eval_twin;
-    }
-    DevR1cs d;
+    cw_r1cs *all = general_twin(r, false);
+    const DevR1cs *d;
     int rc = get_dev_r1cs(all, b->device, b->c, d);
     if (rc) return rc;
     R1csOut eo;
@@ -1604,8 +1599,8 @@ int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, 
     eo.stride = r->data.n_constraints;
     eo.first = first;
     eo.count = count;
-    CU(cudaMemsetAsync(b->fb_d, 0xFF, (size_t)b->batch * 8, b->stream));
-    return launch_r1cs(all, d, b->store(), b->stream, b->fb_d, &eo, nullptr);
+    CU(cudaMemsetAsync(b->fb_d.get(), 0xFF, (size_t)b->batch * 8, b->stream.get()));
+    return launch_r1cs(all, *d, b->store(), b->stream.get(), b->fb_d.get(), &eo, nullptr);
 }
 
 // ---- Groth16 quotient evaluations (the QAP step every Groth16 prover starts with) --------------------------------
@@ -1628,57 +1623,29 @@ static int qap_domain(const cw_r1cs *r, u32 &log_n, u32 &n_public) {
     return CW_OK;
 }
 
-// the constraints plus the rows a_{m+j} = 1 * w_j (j <= nPublic), compiled like the eval twin (every row general)
-static cw_r1cs *qap_twin(cw_r1cs *r, u32 n_public) {
-    std::lock_guard<std::mutex> lk(r->mu);
-    if (r->qap_twin) return r->qap_twin;
-    cw_r1cs *t = new cw_r1cs();
-    t->data = r->data;
-    t->F = r->F;
-    t->no_bool_rows = true;
-    R1csData &D = t->data;
-    D.has_custom_gates = false;
-    D.gates_used.clear();
-    D.gates_applied.clear();
-    const U256 one = u256_from_u64(1);
-    u32 one_idx = (u32)D.dict.size();
-    for (size_t i = 0; i < D.dict.size(); ++i)
-        if (D.dict[i] == one) { one_idx = (u32)i; break; }
-    if (one_idx == D.dict.size()) D.dict.push_back(one);
-    for (u32 j = 0; j <= n_public; ++j) {   // row_ptr[3 m] (the end of the last row) is the start of the new row's A block
-        D.col.push_back(j);
-        D.coef.push_back(one_idx);
-        for (int k = 0; k < 3; ++k) D.row_ptr.push_back(D.col.size());
-    }
-    D.n_constraints += n_public + 1;
-    r->qap_twin = t;
-    return t;
-}
-
 // twiddle and coset-scale tables of one (device, prime, log_n), Montgomery images (ntt.cuh: ntt_tables)
 struct NttTables {
-    u32 *tw = nullptr, *shi = nullptr, *slo = nullptr;
+    DevPtr<u32> tw, shi, slo;
 };
 static std::mutex g_ntt_mu;
-static std::map<std::tuple<int, int, u32>, NttTables> g_ntt_tables;   // (device, prime, log_n): kept for the process
+// (device, prime, log_n): kept for the process, and never destroyed (no device calls at exit)
+static auto &g_ntt_tables = *new std::map<std::tuple<int, int, u32>, NttTables>();
 
-static int ntt_tables_for(int device, int prime_id, u32 log_n, NttTables &out) {
+static int ntt_tables_for(int device, int prime_id, u32 log_n, const NttTables *&out) {
     std::lock_guard<std::mutex> lk(g_ntt_mu);
     auto key = std::make_tuple(device, prime_id, log_n);
     auto it = g_ntt_tables.find(key);
-    if (it != g_ntt_tables.end()) {
-        out = it->second;
-        return CW_OK;
+    if (it == g_ntt_tables.end()) {
+        std::vector<U256> tw, shi, slo;
+        ntt_tables(make_field(prime_id), log_n, tw, shi, slo);
+        NttTables t;
+        int rc;
+        if ((rc = upload(t.tw, tw.data(), tw.size() * 32))) return rc;
+        if ((rc = upload(t.shi, shi.data(), shi.size() * 32))) return rc;
+        if ((rc = upload(t.slo, slo.data(), slo.size() * 32))) return rc;
+        it = g_ntt_tables.emplace(key, std::move(t)).first;
     }
-    std::vector<U256> tw, shi, slo;
-    ntt_tables(make_field(prime_id), log_n, tw, shi, slo);
-    NttTables t;
-    int rc;
-    if ((rc = upload(&t.tw, tw.data(), tw.size() * 32))) return rc;
-    if ((rc = upload(&t.shi, shi.data(), shi.size() * 32))) return rc;
-    if ((rc = upload(&t.slo, slo.data(), slo.size() * 32))) return rc;
-    g_ntt_tables[key] = t;
-    out = t;
+    out = &it->second;
     return CW_OK;
 }
 
@@ -1694,14 +1661,14 @@ static int launch_ntt_passes(const NttPass *ps, u32 np, bool dit, const NttVecs 
         const NttPass &p = ps[k];
         const u32 tiles = 1u << (p.log_n - p.b - p.log_g);
         dim3 grid(tiles, std::min<u32>(V.n_vec, 65535u));
-        kern<<<grid, NTT_THREADS, (size_t)32 << (p.b + p.log_g), stream>>>(p, V, tb.tw, tb.shi, tb.slo, prime);
+        kern<<<grid, NTT_THREADS, (size_t)32 << (p.b + p.log_g), stream>>>(p, V, tb.tw.get(), tb.shi.get(), tb.slo.get(), prime);
     }
     return CW_OK;
 }
 
 // the vectors of V (d0 + v n for v < n0, then d1) through one transform of mode NTT_MODE_*, on `stream`
 static int run_ntt(int device, int prime_id, u32 log_n, const NttVecs &V, int mode, cudaStream_t stream) {
-    NttTables tb;
+    const NttTables *tb;
     int rc = ntt_tables_for(device, prime_id, log_n, tb);
     if (rc) return rc;
     NttPass dif[NTT_MAX_PASSES], dit[NTT_MAX_PASSES];
@@ -1709,9 +1676,9 @@ static int run_ntt(int device, int prime_id, u32 log_n, const NttVecs &V, int mo
     const u32 scale = mode == NTT_MODE_FORWARD ? NTT_SCALE_NONE : mode == NTT_MODE_INVERSE ? NTT_SCALE_CONST : NTT_SCALE_COSET;
     const u32 nd = ntt_plan(log_n, false, mode != NTT_MODE_FORWARD, scale, lg_lo, dif);
     const u32 nt = mode == NTT_MODE_COSET ? ntt_plan(log_n, true, 0u, NTT_SCALE_NONE, lg_lo, dit) : 0u;
-    if ((rc = launch_ntt_passes(dif, nd, false, V, tb, prime_id, stream))) return rc;
+    if ((rc = launch_ntt_passes(dif, nd, false, V, *tb, prime_id, stream))) return rc;
     if (mode == NTT_MODE_COSET) {
-        if ((rc = launch_ntt_passes(dit, nt, true, V, tb, prime_id, stream))) return rc;
+        if ((rc = launch_ntt_passes(dit, nt, true, V, *tb, prime_id, stream))) return rc;
     } else {
         const u32 n = 1u << log_n;
         dim3 grid(std::max<u32>(1u, std::min<u32>((n + 255) / 256, device_sms() * 8)), std::min<u32>(V.n_vec, 65535u));
@@ -1737,8 +1704,8 @@ static int quotient_on_store(cw_r1cs *r, int device, const cw_circuit *layout, c
     u32 k = 0, np = 0;
     int rc = qap_domain(r, k, np);
     if (rc) return rc;
-    cw_r1cs *t = qap_twin(r, np);
-    DevR1cs d;
+    cw_r1cs *t = general_twin(r, true, np);
+    const DevR1cs *d;
     if ((rc = get_dev_r1cs(t, device, layout, d))) return rc;
     const uint64_t n = 1ull << k, rows = t->data.n_constraints;
     uint4 *A = (uint4 *)h_dev, *B = (uint4 *)scratch_dev, *Cc = B + 2 * (size_t)count * n;
@@ -1752,7 +1719,7 @@ static int quotient_on_store(cw_r1cs *r, int device, const cw_circuit *layout, c
     eo.first = first;
     eo.count = count;
     eo.ab = true;
-    if ((rc = launch_r1cs(t, d, S, stream, fb_d, &eo, nullptr))) return rc;
+    if ((rc = launch_r1cs(t, *d, S, stream, fb_d, &eo, nullptr))) return rc;
     NttVecs V;
     V.d0 = A;
     V.d1 = B;
@@ -1775,8 +1742,8 @@ int cw_r1cs_quotient_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t cou
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     if (r->data.prime_id != b->c->tape.F.prime_id) return fail(CW_EINVAL, "the R1CS and the batch use different primes");
     CU(cudaSetDevice(b->device));
-    CU(cudaMemsetAsync(b->fb_d, 0xFF, (size_t)b->batch * 8, b->stream));
-    return quotient_on_store(r, b->device, b->c, b->store(), first, count, h_dev, scratch_dev, b->fb_d, b->stream);
+    CU(cudaMemsetAsync(b->fb_d.get(), 0xFF, (size_t)b->batch * 8, b->stream.get()));
+    return quotient_on_store(r, b->device, b->c, b->store(), first, count, h_dev, scratch_dev, b->fb_d.get(), b->stream.get());
 }
 
 int cw_r1cs_quotient_strided(cw_r1cs *r, const uint64_t *witness_dev, uint64_t stride_elems, uint32_t count, int device,
@@ -1787,22 +1754,13 @@ int cw_r1cs_quotient_strided(cw_r1cs *r, const uint64_t *witness_dev, uint64_t s
         return fail(CW_EINVAL, "device pointers must be 32-byte aligned");
     int rc = ensure_device(device);
     if (rc) return rc;
-    StoreDev S;
-    S.slots = (const uint4 *)witness_dev;
-    S.plane = nullptr;
-    S.n_slots = (u32)stride_elems;
-    S.n_bitwords = 0;
-    S.bt_log2 = 0;
-    S.batch = count;
-    unsigned long long *fb_d = nullptr;
-    CU(cudaMalloc((void **)&fb_d, (size_t)count * 8));
-    rc = quotient_on_store(r, device, nullptr, S, 0, count, h_dev, scratch_dev, fb_d, 0);
-    if (!rc) {
-        cudaError_t e = cudaStreamSynchronize(0);
-        if (e != cudaSuccess) rc = fail(CW_ECUDA, cudaGetErrorString(e));
-    }
-    cudaFree(fb_d);
-    return rc;
+    DevPtr<unsigned long long> fb_d;
+    if ((rc = dev_alloc(fb_d, (size_t)count * 8))) return rc;
+    if ((rc = quotient_on_store(r, device, nullptr, dense_store(witness_dev, stride_elems, count), 0, count, h_dev, scratch_dev,
+                                fb_d.get(), 0)))
+        return rc;
+    CU(cudaStreamSynchronize(0));
+    return CW_OK;
 }
 
 int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *data_dev, int mode, int device) {
@@ -1830,7 +1788,7 @@ int cw_fr_ntt_batch(int prime_id, uint32_t log2_n, uint32_t count, uint64_t *dat
 struct cw_g1_bases {
     int device = 0;
     uint64_t n = 0;
-    u32 *pts = nullptr;   // [n][16] u32: Montgomery x, y; (0, 0) = infinity
+    DevPtr<u32> pts;   // [n][16] u32: Montgomery x, y; (0, 0) = infinity
 };
 
 static const uint64_t MSM_MAX_N = 1ull << 26;
@@ -1920,21 +1878,17 @@ int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int dev
     }
     int rc = ensure_device(device);
     if (rc) return rc;
-    cw_g1_bases *b = new cw_g1_bases();
+    auto b = std::make_unique<cw_g1_bases>();
     b->device = device;
     b->n = n;
-    if ((rc = upload(&b->pts, mont.data(), (size_t)n * 64))) {
-        delete b;
-        return rc;
-    }
-    *out = b;
+    if ((rc = upload(b->pts, mont.data(), (size_t)n * 64))) return rc;
+    *out = b.release();
     return CW_OK;
 }
 
 void cw_g1_bases_destroy(cw_g1_bases *b) {
     if (!b) return;
     cudaSetDevice(b->device);
-    cudaFree(b->pts);
     delete b;
 }
 
@@ -2009,7 +1963,7 @@ int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride
         uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
         int lv = 0;
         msm_runs_kernel<true><<<(u32)((threads + MSM_THREADS - 1) / MSM_THREADS), MSM_THREADS, 0, st>>>(
-            k1, v1, b->pts, nullptr, N, p.c, buckets, (u32 *)(S + p.lv_keys[0]), (Xyzz *)(S + p.lv_pts[0]));
+            k1, v1, b->pts.get(), nullptr, N, p.c, buckets, (u32 *)(S + p.lv_keys[0]), (Xyzz *)(S + p.lv_pts[0]));
         while (threads > 1) {
             items = msm_level_out(items);
             threads = (items + MSM_RUN - 1) / MSM_RUN;
@@ -2033,7 +1987,7 @@ int cw_g1_msm_batch(cw_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride
 struct cw_g2_bases {
     int device = 0;
     uint64_t n = 0;
-    u32 *pts = nullptr;   // [n][32] u32: Montgomery x.c0, x.c1, y.c0, y.c1; all zeros = infinity
+    DevPtr<u32> pts;   // [n][32] u32: Montgomery x.c0, x.c1, y.c0, y.c1; all zeros = infinity
 };
 
 // b' = 3 / (9 + u), canonical (c0, c1)
@@ -2086,21 +2040,17 @@ int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int dev
     }
     int rc = ensure_device(device);
     if (rc) return rc;
-    cw_g2_bases *b = new cw_g2_bases();
+    auto b = std::make_unique<cw_g2_bases>();
     b->device = device;
     b->n = n;
-    if ((rc = upload(&b->pts, mont.data(), (size_t)n * 128))) {
-        delete b;
-        return rc;
-    }
-    *out = b;
+    if ((rc = upload(b->pts, mont.data(), (size_t)n * 128))) return rc;
+    *out = b.release();
     return CW_OK;
 }
 
 void cw_g2_bases_destroy(cw_g2_bases *b) {
     if (!b) return;
     cudaSetDevice(b->device);
-    cudaFree(b->pts);
     delete b;
 }
 
@@ -2135,7 +2085,7 @@ int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride
         // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
         uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
         int lv = 0;
-        msm_g2_launch_runs(true, (const u32 *)(S + p.keys[1]), (const u32 *)(S + p.vals[1]), b->pts, nullptr, N, p.c, buckets,
+        msm_g2_launch_runs(true, (const u32 *)(S + p.keys[1]), (const u32 *)(S + p.vals[1]), b->pts.get(), nullptr, N, p.c, buckets,
                            (u32 *)(S + p.lv_keys[0]), S + p.lv_pts[0], st);
         while (threads > 1) {
             items = msm_level_out(items);
@@ -2173,24 +2123,20 @@ int cw_wtns_read(const char *path, int *prime_id, uint64_t *n_witness, uint64_t 
 // constraint holds, else the smallest violated row
 int cw_r1cs_check_files(const char *r1cs_path, const char *wtns_path, int device, int64_t *first_bad) {
     if (!r1cs_path || !wtns_path || !first_bad) return fail(CW_EINVAL, "null argument");
-    cw_r1cs *r = nullptr;
-    int rc = cw_r1cs_load(r1cs_path, &r);
+    cw_r1cs *loaded = nullptr;
+    int rc = cw_r1cs_load(r1cs_path, &loaded);
     if (rc) return rc;
+    std::unique_ptr<cw_r1cs, void (*)(cw_r1cs *)> r(loaded, cw_r1cs_destroy);
     std::vector<uint64_t> w;
     int pid = 0;
     try {
         read_wtns(wtns_path, pid, w);
     } catch (const std::exception &e) {
-        cw_r1cs_destroy(r);
         return fail(CW_EFORMAT, e.what());
     }
-    if (pid != r->data.prime_id || w.size() / 4 != r->data.n_wires) {
-        cw_r1cs_destroy(r);
+    if (pid != r->data.prime_id || w.size() / 4 != r->data.n_wires)
         return fail(CW_EINVAL, "the witness and the constraint system do not match (prime or number of wires)");
-    }
-    rc = cw_r1cs_check(r, w.data(), 0, 1, device, first_bad, nullptr);
-    cw_r1cs_destroy(r);
-    return rc;
+    return cw_r1cs_check(r.get(), w.data(), 0, 1, device, first_bad, nullptr);
 }
 
 // ---- lowered circuit as a blob / multi-GPU plumbing -----------------------------------------------------------
@@ -2207,14 +2153,13 @@ int cw_circuit_serialize(const cw_circuit *c, uint8_t *out, size_t cap, size_t *
 
 int cw_circuit_deserialize(const void *data, size_t len, cw_circuit **out) {
     if (!data || !out) return fail(CW_EINVAL, "null argument");
-    cw_circuit *c = new cw_circuit();
+    auto c = std::make_unique<cw_circuit>();
     try {
         deserialize_tape((const uint8_t *)data, len, c->tape);
     } catch (const std::exception &e) {
-        delete c;
         return fail(CW_EFORMAT, e.what());
     }
-    *out = c;
+    *out = c.release();
     return CW_OK;
 }
 
@@ -2225,7 +2170,6 @@ int cw_batch_pack_device(cw_batch *b, uint32_t first, uint32_t count, uint32_t *
     if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
     CU(cudaSetDevice(b->device));
     const PackLayout &L = b->c->pack_layout();
-    if (!b->pack_flag_d) CU(cudaMalloc((void **)&b->pack_flag_d, 4));
     return pack_rows(b, L, first, count, dst_device);
 }
 
@@ -2288,7 +2232,7 @@ struct cw_comm {
     ncclComm_t comm = nullptr;
     int rank = 0, world = 1, device = 0;
     bool owned = false;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     uint64_t bytes_sent = 0, bytes_received = 0;  // payload bytes this rank moved through the data-path collectives
 };
 
@@ -2310,18 +2254,15 @@ int cw_comm_init(const uint8_t id[CW_COMM_ID_BYTES], int rank, int world, int de
     if ((rc = ensure_device(device))) return rc;
     ncclUniqueId u;
     memcpy(&u, id, sizeof(u));
-    cw_comm *c = new cw_comm();
+    auto c = std::make_unique<cw_comm>();
     c->rank = rank;
     c->world = world;
     c->device = device;
-    c->owned = true;
+    if ((rc = make_stream(c->stream))) return rc;   // (before the communicator: nothing can fail after it exists)
     ncclResult_t r = g_nccl.CommInitRank(&c->comm, world, u, rank);
-    if (r != ncclSuccess) {
-        delete c;
-        return fail(CW_ECUDA, std::string("ncclCommInitRank: ") + g_nccl.GetErrorString(r));
-    }
-    CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    *out = c;
+    if (r != ncclSuccess) return fail(CW_ECUDA, std::string("ncclCommInitRank: ") + g_nccl.GetErrorString(r));
+    c->owned = true;
+    *out = c.release();
     return CW_OK;
 }
 
@@ -2330,23 +2271,20 @@ int cw_comm_from_nccl(void *nccl_comm, int rank, int world, int device, cw_comm 
     int rc = load_nccl();
     if (rc) return rc;
     if ((rc = ensure_device(device))) return rc;
-    cw_comm *c = new cw_comm();
+    auto c = std::make_unique<cw_comm>();
     c->comm = (ncclComm_t)nccl_comm;
     c->rank = rank;
     c->world = world;
     c->device = device;
-    CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    *out = c;
+    if ((rc = make_stream(c->stream))) return rc;
+    *out = c.release();
     return CW_OK;
 }
 
 void cw_comm_destroy(cw_comm *c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) {
-        cudaStreamSynchronize(c->stream);
-        cudaStreamDestroy(c->stream);
-    }
+    if (c->stream) cudaStreamSynchronize(c->stream.get());
     if (c->owned && c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
     delete c;
 }
@@ -2366,26 +2304,26 @@ int cw_circuit_broadcast(cw_comm *cm, cw_circuit **c, int root) {
     CU(cudaSetDevice(cm->device));
     std::vector<uint8_t> blob;
     if (cm->rank == root) serialize_tape((*c)->tape, blob);
-    unsigned long long n = blob.size(), *n_d = nullptr;
-    CU(cudaMalloc((void **)&n_d, 8));
-    CU(cudaMemcpy(n_d, &n, 8, cudaMemcpyHostToDevice));
-    NC(g_nccl.Broadcast(n_d, n_d, 8, ncclUint8, root, cm->comm, cm->stream));
-    CU(cudaStreamSynchronize(cm->stream));
-    CU(cudaMemcpy(&n, n_d, 8, cudaMemcpyDeviceToHost));
-    cudaFree(n_d);
-    uint8_t *buf_d = nullptr;
-    CU(cudaMalloc((void **)&buf_d, n ? n : 16));
-    if (cm->rank == root) CU(cudaMemcpy(buf_d, blob.data(), n, cudaMemcpyHostToDevice));
-    NC(g_nccl.Broadcast(buf_d, buf_d, n, ncclUint8, root, cm->comm, cm->stream));
-    CU(cudaStreamSynchronize(cm->stream));
-    int rc = CW_OK;
-    if (cm->rank != root) {
-        blob.resize(n);
-        CU(cudaMemcpy(blob.data(), buf_d, n, cudaMemcpyDeviceToHost));
-        rc = cw_circuit_deserialize(blob.data(), blob.size(), c);
-        cm->bytes_received += n;
-    } else cm->bytes_sent += n * (uint64_t)(cm->world - 1);
-    cudaFree(buf_d);
+    unsigned long long n = blob.size();
+    DevPtr<unsigned long long> n_d;
+    int rc;
+    if ((rc = upload(n_d, &n, 8))) return rc;
+    NC(g_nccl.Broadcast(n_d.get(), n_d.get(), 8, ncclUint8, root, cm->comm, cm->stream.get()));
+    CU(cudaStreamSynchronize(cm->stream.get()));
+    CU(cudaMemcpy(&n, n_d.get(), 8, cudaMemcpyDeviceToHost));
+    DevPtr<uint8_t> buf_d;
+    if ((rc = dev_alloc(buf_d, n ? n : 16))) return rc;
+    if (cm->rank == root) CU(cudaMemcpy(buf_d.get(), blob.data(), n, cudaMemcpyHostToDevice));
+    NC(g_nccl.Broadcast(buf_d.get(), buf_d.get(), n, ncclUint8, root, cm->comm, cm->stream.get()));
+    CU(cudaStreamSynchronize(cm->stream.get()));
+    if (cm->rank == root) {
+        cm->bytes_sent += n * (uint64_t)(cm->world - 1);
+        return CW_OK;
+    }
+    blob.resize(n);
+    CU(cudaMemcpy(blob.data(), buf_d.get(), n, cudaMemcpyDeviceToHost));
+    rc = cw_circuit_deserialize(blob.data(), blob.size(), c);
+    cm->bytes_received += n;
     return rc;
 }
 
@@ -2403,26 +2341,23 @@ int cw_batch_gather_witness_packed(cw_comm *cm, cw_batch *b, uint32_t first, uin
     CU(cudaSetDevice(b->device));
     const PackLayout &L = b->c->pack_layout();
     const size_t n = (size_t)count * L.words * 4;  // bytes per rank
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
-    CU(cudaEventRecord(e0, b->stream));
+    Event e0, e1;
+    int rc;
+    if ((rc = make_event(e0)) || (rc = make_event(e1))) return rc;
+    CU(cudaEventRecord(e0.get(), b->stream.get()));
     uint32_t *mine = cm->rank == root ? recv_device + (size_t)root * count * L.words : send_scratch_device;
-    int rc = cw_batch_pack_device(b, first, count, mine);
-    if (rc) return rc;
+    if ((rc = cw_batch_pack_device(b, first, count, mine))) return rc;
     NC(g_nccl.GroupStart());
     if (cm->rank == root) {
         for (int r = 0; r < cm->world; ++r)
-            if (r != root) NC(g_nccl.Recv(recv_device + (size_t)r * count * L.words, n, ncclUint8, r, cm->comm, b->stream));
+            if (r != root) NC(g_nccl.Recv(recv_device + (size_t)r * count * L.words, n, ncclUint8, r, cm->comm, b->stream.get()));
     } else {
-        NC(g_nccl.Send(mine, n, ncclUint8, root, cm->comm, b->stream));
+        NC(g_nccl.Send(mine, n, ncclUint8, root, cm->comm, b->stream.get()));
     }
     NC(g_nccl.GroupEnd());
-    CU(cudaEventRecord(e1, b->stream));
-    CU(cudaStreamSynchronize(b->stream));
-    if (ms) CU(cudaEventElapsedTime(ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
+    CU(cudaEventRecord(e1.get(), b->stream.get()));
+    CU(cudaStreamSynchronize(b->stream.get()));
+    if (ms) CU(cudaEventElapsedTime(ms, e0.get(), e1.get()));
     if (cm->rank == root) cm->bytes_received += n * (uint64_t)(cm->world - 1);
     else cm->bytes_sent += n;
     return CW_OK;
@@ -2435,17 +2370,17 @@ int cw_status_allreduce(cw_comm *cm, cw_batch *b, uint64_t out[2]) {
     std::vector<int32_t> st(b->batch);
     int rc = cw_batch_status(b, st.data());
     if (rc) return rc;
-    unsigned long long h[2] = {0, 0}, *d = nullptr;
+    unsigned long long h[2] = {0, 0};
     for (int32_t s : st) {
         if (s > 0) ++h[0];
         else if (s < 0) ++h[1];
     }
-    CU(cudaMalloc((void **)&d, 16));
-    CU(cudaMemcpyAsync(d, h, 16, cudaMemcpyHostToDevice, b->stream));
-    NC(g_nccl.AllReduce(d, d, 2, ncclUint64, ncclSum, cm->comm, b->stream));
-    CU(cudaMemcpyAsync(h, d, 16, cudaMemcpyDeviceToHost, b->stream));
-    CU(cudaStreamSynchronize(b->stream));
-    cudaFree(d);
+    DevPtr<unsigned long long> d;
+    if ((rc = dev_alloc(d, 16))) return rc;
+    CU(cudaMemcpyAsync(d.get(), h, 16, cudaMemcpyHostToDevice, b->stream.get()));
+    NC(g_nccl.AllReduce(d.get(), d.get(), 2, ncclUint64, ncclSum, cm->comm, b->stream.get()));
+    CU(cudaMemcpyAsync(h, d.get(), 16, cudaMemcpyDeviceToHost, b->stream.get()));
+    CU(cudaStreamSynchronize(b->stream.get()));
     out[0] = h[0];
     out[1] = h[1];
     return CW_OK;
@@ -2457,28 +2392,23 @@ int cw_fr_batch_op(int prime_id, int op, const uint64_t *a, const uint64_t *b, c
     if (!a || !r || prime_id < 0 || prime_id >= CW_N_PRIMES) return fail(CW_EINVAL, "bad argument");
     int rc = ensure_device(device);
     if (rc) return rc;
-    uint4 *A = nullptr, *B = nullptr, *C = nullptr, *Rr = nullptr;
-    int *err = nullptr;
-    if ((rc = upload(&A, a, n * 32))) return rc;
-    if (b && (rc = upload(&B, b, n * 32))) return rc;
-    if (c && (rc = upload(&C, c, n * 32))) return rc;
-    CU(cudaMalloc((void **)&Rr, n * 32 + 32));
-    CU(cudaMalloc((void **)&err, 4));
-    CU(cudaMemset(err, 0, 4));
+    DevPtr<uint4> A, B, C, Rr;
+    DevPtr<int> err;
+    if ((rc = upload(A, a, n * 32))) return rc;
+    if (b && (rc = upload(B, b, n * 32))) return rc;
+    if (c && (rc = upload(C, c, n * 32))) return rc;
+    if ((rc = dev_alloc(Rr, n * 32 + 32))) return rc;
+    if ((rc = dev_alloc(err, 4))) return rc;
+    CU(cudaMemset(err.get(), 0, 4));
     u32 grid = (u32)std::min<size_t>((n + 127) / 128, device_sms() * 16);
     if (!grid) grid = 1;
-    if (prime_id == 0) fr_batch_op_kernel<0><<<grid, 128>>>(op, A, B, C, Rr, n, err, 0u);
-    else if (prime_id == 1) fr_batch_op_kernel<1><<<grid, 128>>>(op, A, B, C, Rr, n, err, 1u);
-    else fr_batch_op_kernel<-1><<<grid, 128>>>(op, A, B, C, Rr, n, err, (u32)prime_id);
+    if (prime_id == 0) fr_batch_op_kernel<0><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), 0u);
+    else if (prime_id == 1) fr_batch_op_kernel<1><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), 1u);
+    else fr_batch_op_kernel<-1><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), (u32)prime_id);
     CU(cudaGetLastError());
-    CU(cudaMemcpy(r, Rr, n * 32, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(r, Rr.get(), n * 32, cudaMemcpyDeviceToHost));
     int herr = 0;
-    CU(cudaMemcpy(&herr, err, 4, cudaMemcpyDeviceToHost));
-    cudaFree(A);
-    cudaFree(B);
-    cudaFree(C);
-    cudaFree(Rr);
-    cudaFree(err);
+    CU(cudaMemcpy(&herr, err.get(), 4, cudaMemcpyDeviceToHost));
     return herr ? fail(CW_EINVAL, "division by zero in batch op") : CW_OK;
 }
 
@@ -2493,23 +2423,18 @@ int cw_fr_mul_bench(int prime_id, size_t n, int iters, int device, float *ms) {
         x = s;
     }
     for (size_t i = 0; i < n; ++i) h[4 * i + 3] &= 0x0FFFFFFFFFFFFFFFull;
-    uint4 *d = nullptr;
-    if ((rc = upload(&d, h.data(), n * 32))) return rc;
-    cudaEvent_t e0, e1;
-    CU(cudaEventCreate(&e0));
-    CU(cudaEventCreate(&e1));
+    DevPtr<uint4> d;
+    Event e0, e1;
+    if ((rc = upload(d, h.data(), n * 32)) || (rc = make_event(e0)) || (rc = make_event(e1))) return rc;
     u32 grid = (u32)((n + 255) / 256);
     for (int rep = 0; rep < 2; ++rep) {
-        CU(cudaEventRecord(e0));
-        if (prime_id == 0) fr_mul_bench_kernel<0><<<grid, 256>>>(d, n, iters);
-        else fr_mul_bench_kernel<1><<<grid, 256>>>(d, n, iters);
-        CU(cudaEventRecord(e1));
-        CU(cudaEventSynchronize(e1));
+        CU(cudaEventRecord(e0.get()));
+        if (prime_id == 0) fr_mul_bench_kernel<0><<<grid, 256>>>(d.get(), n, iters);
+        else fr_mul_bench_kernel<1><<<grid, 256>>>(d.get(), n, iters);
+        CU(cudaEventRecord(e1.get()));
+        CU(cudaEventSynchronize(e1.get()));
     }
-    CU(cudaEventElapsedTime(ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    cudaFree(d);
+    CU(cudaEventElapsedTime(ms, e0.get(), e1.get()));
     return CW_OK;
 }
 

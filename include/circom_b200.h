@@ -157,6 +157,7 @@ int cw_circuit_write_dat(const cw_circuit *c, const char *path);
 int cw_circuit_write_sym(const cw_circuit *c, const char *path);
 
 /* ---- batch: Circom_CalcWit for `batch` independent inputs on one GPU ------------------------ */
+/* a batch uses its circuit on every call: destroy every batch of a circuit before the circuit */
 int cw_batch_create(const cw_circuit *c, uint32_t batch, int device, cw_batch **out);
 void cw_batch_destroy(cw_batch *b);
 /* how the batch lays its values out on the device: log2 of the instances per tile (0: one instance per CTA, lanes
