@@ -42,6 +42,9 @@ def lib():
         _lib.orc_free.argtypes = [ctypes.c_void_p]
         _lib.orc_run_many.restype = ctypes.c_long
         _lib.orc_run_many.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_long, ctypes.c_int]
+        _lib.orc_poly_eval.restype = ctypes.c_int
+        _lib.orc_poly_eval.argtypes = [ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_void_p, ctypes.c_int,
+                                       ctypes.c_void_p]
     return _lib
 
 
@@ -87,6 +90,17 @@ class COracle:
         witness = np.ascontiguousarray(witness, dtype=np.uint64).reshape(-1, self.n_signals, 4)
         return np.array([lib().orc_r1cs_check(self._h, witness[i].ctypes.data) for i in range(witness.shape[0])],
                         dtype=np.int64)
+
+
+def poly_eval(prime_id: int, coef: np.ndarray, x: int, threads: int = 0) -> int:
+    """sum_i coef[i] x^i mod q for canonical coefficients uint64 [n][4] (Horner's rule on `threads` threads, 0: one per
+    CPU)"""
+    coef = np.ascontiguousarray(coef, dtype=np.uint64).reshape(-1, 4)
+    xs = (ctypes.c_uint64 * 4)(*[(x >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)])
+    r = (ctypes.c_uint64 * 4)()
+    if not lib().orc_poly_eval(prime_id, coef.ctypes.data, coef.shape[0], xs, threads or os.cpu_count() or 1, r):
+        raise ValueError("unknown prime id %d" % prime_id)
+    return sum(int(r[i]) << (64 * i) for i in range(4))
 
 
 def apply(prime_id: int, op: int, a: int, b: int = 0, c: int = 0) -> int:

@@ -558,6 +558,48 @@ long orc_run_many(const circuit *c, const u64 *inputs, long n, int threads) {
     return ok;
 }
 
+/* ---- polynomial evaluation, for spot checks of transforms too large for a Python sum: out = sum_{i<n} coef[i] x^i
+ * (coef[n][4] and x canonical, below q).  Horner's rule over `threads` contiguous slices of the coefficients; slice t
+ * starting at lo contributes x^lo times its own Horner value.  Returns 0 for an unknown prime. */
+typedef struct { const field_t *F; const fe *coef; u64 lo, hi; fe xm, acc; } horner_t;
+static void *horner_worker(void *p) {
+    horner_t *h = (horner_t *)p;
+    fe acc = fe_u64(0), t;
+    for (u64 i = h->hi; i-- > h->lo;) {
+        f_mmul(h->F, &t, &acc, &h->xm);   /* acc * x: the Montgomery image of x times a normal value is normal */
+        f_add(h->F, &acc, &t, &h->coef[i]);
+    }
+    h->acc = acc;
+    return NULL;
+}
+int orc_poly_eval(u32 prime, const u64 *coef, u64 n, const u64 *x, int threads, u64 *out) {
+    if (prime >= 8) return 0;
+    field_t F;
+    field_init(&F, prime);
+    if (threads < 1) threads = 1;
+    if ((u64)threads > n) threads = n ? (int)n : 1;
+    pthread_t *th = (pthread_t *)malloc(sizeof(pthread_t) * threads);
+    horner_t *hs = (horner_t *)calloc(threads, sizeof(horner_t));
+    fe xm;
+    f_mmul(&F, &xm, (const fe *)x, &F.r2);
+    for (int t = 0; t < threads; ++t) {
+        hs[t].F = &F; hs[t].coef = (const fe *)coef; hs[t].xm = xm;
+        hs[t].lo = n * t / threads; hs[t].hi = n * (t + 1) / threads;
+        pthread_create(&th[t], NULL, horner_worker, &hs[t]);
+    }
+    fe sum = fe_u64(0);
+    for (int t = 0; t < threads; ++t) {
+        pthread_join(th[t], NULL);
+        fe e = fe_u64(hs[t].lo), xl, p;
+        f_pow(&F, &xl, (const fe *)x, &e);
+        f_mul(&F, &p, &hs[t].acc, &xl);
+        f_add(&F, &sum, &sum, &p);
+    }
+    memcpy(out, sum.v, 32);
+    free(th); free(hs);
+    return 1;
+}
+
 void orc_free(circuit *c) {
     if (!c) return;
     for (u32 i = 0; i < c->n_tm; ++i) { free(c->tm[i].subs); free(c->tm[i].ops); free(c->tm[i].lc_len); free(c->tm[i].terms); }

@@ -86,3 +86,23 @@ def test_reference_runtime_wtns_equals_oracle(name):
             ir_eval.LOG_SINK.clear()
             evaluate(d, ins[i])
             assert "".join(ir_eval.LOG_SINK) == printed and printed.count("\n") == 4
+
+
+@pytest.mark.parametrize("name", ["bn128", "pallas", "goldilocks"])
+def test_poly_eval_equals_the_model_transform(name):
+    """orc_poly_eval (the evaluator behind the spot checks of large transforms) at the domain points: sum_i x_i w^(ij) is
+    the forward transform of the model, for slice counts that do and do not divide n, and x = 0 / 1"""
+    from oracle import qap_model as QM
+    q, pid = QM.PRIMES[name], QM.PRIME_IDS[name]
+    rng = random.Random(name)
+    for k in (1, 3, 6, 9):
+        n = 1 << k
+        x = [rng.randrange(q) for _ in range(n)]
+        coef = np.array([[(v >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)] for v in x], dtype=np.uint64)
+        want = QM.ntt(x, q)
+        w = QM.root(q, k)
+        for threads in (1, 3, 8):
+            for j in sorted({0, 1, n // 2, n - 1}):
+                assert c_oracle.poly_eval(pid, coef, pow(w, j, q), threads) == want[j], (k, threads, j)
+        assert c_oracle.poly_eval(pid, coef, 0, 5) == x[0]
+        assert c_oracle.poly_eval(pid, coef, 1, 5) == sum(x) % q
