@@ -95,29 +95,6 @@ int upload(DevPtr<T> &dst, const void *src, size_t bytes) {
     return CW_OK;
 }
 
-FrParams make_dev_params(const FieldParams &F) {
-    FrParams p;
-    memset(&p, 0, sizeof(p));
-    auto split = [](u32 *dst, const U256 &v) {
-        for (int i = 0; i < 4; ++i) {
-            dst[2 * i] = (u32)v.v[i];
-            dst[2 * i + 1] = (u32)(v.v[i] >> 32);
-        }
-    };
-    split(p.q, F.q);
-    split(p.half, F.half);
-    split(p.r1, F.r1);
-    split(p.r2, F.r2);
-    U256 two = u256_from_u64(2), qm2;
-    u256_sub(qm2, F.q, two);
-    split(p.qm2, qm2);
-    p.np32 = F.np32;
-    p.qbits = F.qbits;
-    // lboMask of the limb that holds the top bit; fr_mask_wrap clears the limbs above it (goldilocks: limb 1, all ones)
-    p.top_mask = (F.qbits % 32 == 0) ? 0xFFFFFFFFu : ((1u << (F.qbits % 32)) - 1u);
-    return p;
-}
-
 std::mutex g_dev_mutex;
 std::map<int, bool> g_dev_ready;
 
@@ -154,6 +131,15 @@ u32 device_sms() {
     return (u32)n;
 }
 
+// Grid of a grid-stride kernel: CTAs of `threads` for `items`, at most `ctas_per_sm` per SM and at least one.  With `rows`
+// the kernel strides over that many instances, tiles or vectors in y, where a grid ends at 65,535.
+u32 grid_for(uint64_t items, u32 threads, u32 ctas_per_sm) {
+    return (u32)std::max<uint64_t>(1, std::min<uint64_t>((items + threads - 1) / threads, (uint64_t)device_sms() * ctas_per_sm));
+}
+dim3 grid_for(uint64_t items, u32 threads, u32 ctas_per_sm, u32 rows) {
+    return dim3(grid_for(items, threads, ctas_per_sm), std::min<u32>(rows, 65535u));
+}
+
 struct DevTape {
     DevPtr<uint4> ops;
     DevPtr<u32> items, level_start, level_info;
@@ -161,9 +147,10 @@ struct DevTape {
     DevPtr<uint4> heads;  // first tape word of every work item
     DevPtr<uint4> consts;
     DevPtr<u32> input_slot, fn_code, fn_info, call_tab;
-    DevPtr<u32> wloc;  // per witness entry: where its value lives (slot id, or OPD_BIT | plane position)
+    DevPtr<u32> wloc;  // per witness entry: where its value lives (slot id, or OPERAND_BIT | plane position)
     // witness entries outside the bit plane by static size class (slot ids), for the packed device->host transfer
     DevPtr<u32> pk_bit, pk_u64, pk_full;
+    TapeDev view;  // what the kernels take (vm_wide is set per run)
 };
 struct DevR1cs {
     DevPtr<unsigned long long> row_ptr;
@@ -176,6 +163,8 @@ struct DevR1cs {
     u32 n_general = 0, n_bool = 0, n_small = 0;
     u32 mean_row_terms = 0;  // compiled terms per general row
     uint64_t n_terms = 0;
+    R1csDev general, integer;   // what the kernels take: the general rows, the integer rows
+    R1csSmallDev integer_recs;
 };
 
 int env_int(const char *name, int dflt) {
@@ -321,13 +310,13 @@ static int get_dev_tape(const cw_circuit *c, int device, const DevTape *&out) {
             for (uint32_t k = t.level_start[l + 1]; k-- > t.level_start[l];) {
                 const uint32_t opc = t.ops[(size_t)t.items[k] * 4] & 0xFFu;
                 const bool single = t.items[k + 1] - t.items[k] == 1;
-                const bool is_call = opc == 45u && single;
-                if (opc == 45u && !(single && tail)) return fail(CW_ESTATE, "internal: a call is not at the end of its level");
+                const bool is_call = opc == OP_CALL && single;
+                if (opc == OP_CALL && !(single && tail)) return fail(CW_ESTATE, "internal: a call is not at the end of its level");
                 if (is_call) ++info[l];
                 else tail = false;
                 for (uint32_t w = t.items[k]; w < t.items[k + 1]; ++w) {
                     const uint32_t o = t.ops[(size_t)w * 4] & 0xFFu;
-                    if (o == 28u || o == 5u) {   // INV, POW
+                    if (o == OP_INV || o == OP_POW) {
                         if (!single) return fail(CW_ESTATE, "internal: a fused work item contains INV / POW");
                         info[l] |= 0x80000000u;
                         d.has_slow = true;
@@ -346,40 +335,49 @@ static int get_dev_tape(const cw_circuit *c, int device, const DevTape *&out) {
     if ((rc = upload(d.pk_bit, L.bit_loc.data(), L.bit_loc.size() * 4))) return rc;
     if ((rc = upload(d.pk_u64, L.u64_loc.data(), L.u64_loc.size() * 4))) return rc;
     if ((rc = upload(d.pk_full, L.full_loc.data(), L.full_loc.size() * 4))) return rc;
+    TapeDev &tp = d.view;
+    tp.ops = d.ops.get();
+    tp.items = d.items.get();
+    tp.heads = d.heads.get();
+    tp.level_start = d.level_start.get();
+    tp.level_info = d.level_info.get();
+    tp.has_slow = d.has_slow ? 1u : 0u;
+    tp.consts = d.consts.get();
+    tp.n_levels = (u32)t.n_levels();
+    tp.n_slots = t.n_slots;
+    tp.input_slot = d.input_slot.get();
+    tp.fn_code = d.fn_code.get();
+    tp.fn_info = d.fn_info.get();
+    tp.call_tab = d.call_tab.get();
+    tp.n_inputs = (u32)t.n_inputs;
+    tp.n_bitwords = t.n_bitwords;
+    tp.prime = (u32)t.F.prime_id;
+    tp.vm_wide = 0;
     out = &c->dev.emplace(device, std::move(d)).first->second;
     return CW_OK;
 }
 
-// builds of the interpreter: function calls (runtime tile size); fused work items (CW_FLAG_FUSE; runtime tile size, or
-// a warp per op); one operator per work item, per bit-plane mode: one instance per tile / a warp per op (tile sizes
-// fixed at compile time) / tile size as an argument
-// (the fused builds keep their accumulators in dynamic shared memory: kernels.cuh TAPE_ACC_SMEM)
-template <int PR, bool CALLS, bool BP, int BT, bool FU>
-static void launch_tape_k(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th) {
-    constexpr u32 smem = FU ? TAPE_ACC_SMEM : 0u;
-    static_assert(TAPE_ACC_SMEM * CW_TAPE_LB <= 48u * 1024u, "the widest CTA stays within the default dynamic shared memory");
-    tape_exec_kernel<PR, CALLS, BP, BT, FU><<<tiles, th, smem * th, b->stream.get()>>>(
-        tp, b->slots.get(), b->plane.get(), b->bt_log2, b->first_assert_d.get(), b->err_d.get(), b->batch);
+// the build of the interpreter a run of b lands on (tape_calls.h: select_tape_build)
+static int batch_tape_build(const cw_batch *b, TapeBuild &k) {
+    const Tape &t = b->c->tape;
+    if (!select_tape_build(t.F.prime_id, !t.call_tab.empty(), t.n_bitwords != 0, t.n_items() != t.n_tape_ops(), b->bt_log2, k))
+        return fail(CW_ESTATE, "CW_FLAG_FUSE is available for bn128 and bls12381");
+    return CW_OK;
 }
-static void launch_calls(int pr, const TapeDev &tp, cw_batch *b, u32 tiles, u32 th, bool bp, bool fused) {
-    launch_tape_calls(pr, tp, b->slots.get(), b->plane.get(), b->bt_log2, b->first_assert_d.get(), b->err_d.get(), b->batch,
-                      tiles, th, bp, fused, b->stream.get());
-}
-template <int PR>
-static void launch_tape(const TapeDev &tp, cw_batch *b, u32 tiles, u32 th, bool calls, bool bp, bool fused) {
-    if (calls) {  // the builds with the function machine: tape_calls.cu
-        launch_calls(PR, tp, b, tiles, th, bp, fused);
-    } else if (fused) {  // (the bit-plane build also runs tapes without a plane: they contain no plane operands)
-        if (b->bt_log2 == 5) launch_tape_k<PR, false, true, 5, true>(tp, b, tiles, th);
-        else launch_tape_k<PR, false, true, -1, true>(tp, b, tiles, th);
-    } else if (bp) {
-        if (b->bt_log2 == 0) launch_tape_k<PR, false, true, 0, false>(tp, b, tiles, th);
-        else if (b->bt_log2 == 5) launch_tape_k<PR, false, true, 5, false>(tp, b, tiles, th);
-        else launch_tape_k<PR, false, true, -1, false>(tp, b, tiles, th);
-    } else {
-        if (b->bt_log2 == 0) launch_tape_k<PR, false, false, 0, false>(tp, b, tiles, th);
-        else launch_tape_k<PR, false, false, -1, false>(tp, b, tiles, th);
-    }
+
+// the builds without the function machine are compiled here, the others in tape_calls.cu
+static int launch_tape(const TapeBuild &k, const TapeLaunch &a) {
+    const bool found = k.calls ? launch_tape_calls(k, a) : with_prime(k.prime, [&](auto pr) {
+        constexpr int PR = decltype(pr)::value;
+        if constexpr (PR >= 0)
+            return launch_tape_k<PR, false, true, 5, true>(k, a) || launch_tape_k<PR, false, true, -1, true>(k, a) ||
+                   launch_tape_k<PR, false, true, 0, false>(k, a) || launch_tape_k<PR, false, true, 5, false>(k, a) ||
+                   launch_tape_k<PR, false, true, -1, false>(k, a) || launch_tape_k<PR, false, false, 0, false>(k, a) ||
+                   launch_tape_k<PR, false, false, -1, false>(k, a);
+        else
+            return launch_tape_k<-1, false, true, -1, false>(k, a);
+    });
+    return found ? CW_OK : fail(CW_ESTATE, "internal: the library does not contain the interpreter build of this run");
 }
 
 extern "C" {
@@ -660,6 +658,19 @@ int cw_batch_layout(const cw_batch *b, uint32_t *bt_log2, uint32_t *threads, uin
     return CW_OK;
 }
 
+int cw_batch_tape_build(const cw_batch *b, int32_t out[5]) {
+    if (!b || !out) return fail(CW_EINVAL, "null argument");
+    TapeBuild k;
+    int rc = batch_tape_build(b, k);
+    if (rc) return rc;
+    out[0] = k.prime;
+    out[1] = k.calls;
+    out[2] = k.bp;
+    out[3] = k.bt;
+    out[4] = k.fused;
+    return CW_OK;
+}
+
 int cw_batch_set_input(cw_batch *b, uint32_t inst, uint64_t h, uint32_t idx, const uint64_t limbs[4]) {
     if (!b || inst >= b->batch) return fail(CW_EINVAL, "bad instance");
     const Tape &t = b->c->tape;
@@ -718,48 +729,23 @@ int cw_batch_run(cw_batch *b) {
         b->host_inputs_dirty = false;
         b->inputs_on_device = true;
     }
-    TapeDev tp;
-    tp.ops = b->dt->ops.get();
-    tp.items = b->dt->items.get();
-    tp.heads = b->dt->heads.get();
-    tp.level_start = b->dt->level_start.get();
-    tp.level_info = b->dt->level_info.get();
-    tp.has_slow = b->dt->has_slow ? 1u : 0u;
-    tp.consts = b->dt->consts.get();
-    tp.n_levels = (u32)t.n_levels();
-    tp.n_slots = t.n_slots;
-    tp.input_slot = b->dt->input_slot.get();
-    tp.fn_code = b->dt->fn_code.get();
-    tp.fn_info = b->dt->fn_info.get();
-    tp.call_tab = b->dt->call_tab.get();
-    tp.n_inputs = (u32)t.n_inputs;
-    tp.n_bitwords = t.n_bitwords;
-    tp.prime = (u32)t.F.prime_id;
+    TapeDev tp = b->dt->view;
     // the 128-bit register machine computes over the integers and gives up when a value leaves 128 bits: right only for a
     // prime above 2^128 (every 256-bit one); goldilocks calls run on the full-width machine
     tp.vm_wide = (env_int("CW_VM_WIDE", 0) || t.F.qbits <= 128) ? 1u : 0u;
     CU(cudaMemsetAsync(b->first_assert_d.get(), 0xFF, (size_t)b->batch * 4, b->stream.get()));
     CU(cudaMemsetAsync(b->err_d.get(), 0, (size_t)b->batch * 4, b->stream.get()));
     CU(cudaEventRecord(b->ev[0].get(), b->stream.get()));
-    {
-        size_t total = (size_t)b->batch_padded * (t.n_inputs + 1);
-        u32 grid = (u32)std::min<size_t>((total + 255) / 256, device_sms() * 8);
-        stage_inputs_kernel<<<grid, 256, 0, b->stream.get()>>>(tp, b->inputs_d.get(), b->slots.get(), b->batch, b->batch_padded,
-                                                               b->bt_log2);
-    }
-    u32 tiles = b->batch_padded >> b->bt_log2;
+    stage_inputs_kernel<<<grid_for((uint64_t)b->batch_padded * (t.n_inputs + 1), 256, 8), 256, 0, b->stream.get()>>>(
+        tp, b->inputs_d.get(), b->slots.get(), b->batch, b->batch_padded, b->bt_log2);
     if (tp.n_levels) {
-        const bool calls = !t.call_tab.empty();
-        const bool bp = t.n_bitwords != 0;
-        const u32 th = calls ? std::min<u32>(b->threads, 256u) : b->threads;  // the interpreter build has a large frame
-        const bool fused = t.n_items() != t.n_tape_ops();
-        if (t.F.prime_id == 0) launch_tape<0>(tp, b, tiles, th, calls, bp, fused);
-        else if (t.F.prime_id == 1) launch_tape<1>(tp, b, tiles, th, calls, bp, fused);
-        else {  // the other 256-bit primes: one build (bit-plane capable, runtime tile size), prime index from tp.prime
-            if (fused) return fail(CW_ESTATE, "CW_FLAG_FUSE is available for bn128 and bls12381");
-            if (calls) launch_calls(-1, tp, b, tiles, th, true, false);
-            else launch_tape_k<-1, false, true, -1, false>(tp, b, tiles, th);
-        }
+        TapeBuild k;
+        int rc = batch_tape_build(b, k);
+        if (rc) return rc;
+        const u32 th = k.calls ? std::min<u32>(b->threads, 256u) : b->threads;  // the interpreter build has a large frame
+        const TapeLaunch a{tp, b->slots.get(), b->plane.get(), b->bt_log2, b->first_assert_d.get(), b->err_d.get(), b->batch,
+                           b->batch_padded >> b->bt_log2, th, b->stream.get()};
+        if ((rc = launch_tape(k, a))) return rc;
     }
     CU(cudaEventRecord(b->ev[1].get(), b->stream.get()));
     b->dense_valid = false;
@@ -796,8 +782,8 @@ int cw_batch_status(cw_batch *b, int32_t *status) {
 static int expand_rows(cw_batch *b, u32 first, u32 count, uint4 *dst) {
     const Tape &t = b->c->tape;
     if (count == 0) return CW_OK;
-    dim3 grid((u32)std::min<size_t>((t.n_witness + 255) / 256, device_sms() * 4), std::min<u32>(count, 65535u));
-    witness_expand_kernel<<<grid, 256, 0, b->stream.get()>>>(b->store(), b->dt->wloc.get(), (u32)t.n_witness, first, count, dst);
+    witness_expand_kernel<<<grid_for(t.n_witness, 256, 4, count), 256, 0, b->stream.get()>>>(b->store(), b->dt->wloc.get(),
+                                                                                             (u32)t.n_witness, first, count, dst);
     CU(cudaGetLastError());
     return CW_OK;
 }
@@ -866,8 +852,7 @@ static int ensure_pack_buffers(cw_batch *b, const PackLayout &L) {
 // classes (else the proven one, whose location lists are part of the device tape)
 static int pack_rows(cw_batch *b, const PackLayout &L, u32 first, u32 count, u32 *dst_d, const NarrowPack *np = nullptr) {
     const size_t items = L.n_plane_words + L.n_bit_words + L.u64_loc.size() + L.full_loc.size();
-    dim3 grid((u32)std::max<size_t>(1, std::min<size_t>((items + 255) / 256, device_sms() * 4)), std::min<u32>(count, 65535u));
-    witness_pack_kernel<<<grid, 256, 0, b->stream.get()>>>(
+    witness_pack_kernel<<<grid_for(items, 256, 4, count), 256, 0, b->stream.get()>>>(
         b->store(), (np ? np->pk_bit : b->dt->pk_bit).get(), (u32)L.bit_loc.size(), (np ? np->pk_u64 : b->dt->pk_u64).get(),
         (u32)L.u64_loc.size(), (np ? np->pk_full : b->dt->pk_full).get(), (u32)L.full_loc.size(), dst_d, L.words, first, count,
         b->pack_flag_d.get());
@@ -906,8 +891,8 @@ static int observe_classes(cw_batch *b, std::shared_ptr<NarrowPack> prev, std::s
         if ((rc = upload(cls_d, cls.data(), cls.size() * 4))) return rc;
         const u32 n_tiles = (b->batch + (1u << b->bt_log2) - 1) >> b->bt_log2;
         const uint64_t items = (uint64_t)loc.size() << b->bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
-        witness_observe_kernel<<<grid, 256, 0, b->stream.get()>>>(b->store(), loc_d.get(), (u32)loc.size(), cls_d.get());
+        witness_observe_kernel<<<grid_for(items, 256, 8, n_tiles), 256, 0, b->stream.get()>>>(b->store(), loc_d.get(),
+                                                                                              (u32)loc.size(), cls_d.get());
         CU(cudaMemcpyAsync(cls.data(), cls_d.get(), cls.size() * 4, cudaMemcpyDeviceToHost, b->stream.get()));
         CU(cudaStreamSynchronize(b->stream.get()));
         for (size_t k = 0; k < loc.size(); ++k) np->cls[wit[k]] = (uint8_t)std::min<u32>(cls[k], t.wit_class[wit[k]]);
@@ -1304,6 +1289,11 @@ static int compile_r1cs(cw_r1cs *r, const cw_circuit *layout, DevR1cs &d) {
     if ((rc = upload(d.sgroups, h.sgroups.data(), h.sgroups.size() * 4))) return rc;
     if ((rc = upload(d.srecs, h.srecs.data(), h.srecs.size() * sizeof(uint2)))) return rc;
     if ((rc = upload(d.sbrow, h.sbrow.data(), h.sbrow.size() * 4))) return rc;
+    d.general = {d.row_ptr.get(), d.terms.get(), d.dictM.get(), d.perm.get(), d.n_general, (u32)r->data.prime_id};
+    d.integer = d.general;
+    d.integer.perm = d.perm_small.get();
+    d.integer.n_rows = d.n_small;
+    d.integer_recs = {d.sgroups.get(), d.srecs.get(), d.sbrow.get()};
     return CW_OK;
 }
 
@@ -1322,75 +1312,48 @@ static int get_dev_r1cs(cw_r1cs *r, int device, const cw_circuit *layout, const 
     return CW_OK;
 }
 
-struct R1csOut {
-    uint4 *a = nullptr, *b = nullptr, *c = nullptr;
-    uint64_t stride = 0;     // elements between the output rows of consecutive instances
-    u32 first = 0, count = 0;   // instance window of the store
-    bool ab = false;         // c = a o b instead of C.w
-};
-
 // launches on `stream`; fb_d[batch] must hold ~0 on entry; `wide` = (n_small + 31) / 32 + 1 words of scratch for the rows the
 // integer-row kernel hands to the general one
 static int launch_r1cs(cw_r1cs *r, const DevR1cs &d, const StoreDev &S, cudaStream_t stream, unsigned long long *fb_d,
-                       const R1csOut *eval, u32 *wide) {
-    const R1csData &R = r->data;
-    R1csDev rd;
-    rd.row_ptr = d.row_ptr.get();
-    rd.terms = d.terms.get();
-    rd.dictM = d.dictM.get();
-    rd.perm = d.perm.get();
-    rd.n_rows = d.n_general;
-    rd.prime = (u32)R.prime_id;
+                       const EvalOut *eval, u32 *wide) {
+    const int prime_id = r->data.prime_id;
     const u32 bt_mask = (1u << S.bt_log2) - 1u;
     const u32 n_tiles = eval ? ((eval->first + eval->count + bt_mask) >> S.bt_log2) - (eval->first >> S.bt_log2)
                              : (S.batch + bt_mask) >> S.bt_log2;
+    auto grid = [&](u32 rows) { return grid_for((uint64_t)rows << S.bt_log2, 256, 8, n_tiles); };
     if (d.n_general) {
-        const uint64_t items = (uint64_t)d.n_general << S.bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
+        const dim3 g = grid(d.n_general);
         // long rows: many resident warps (48 registers); short rows: the unspilled build
         const bool lean = env_int("CW_R1CS_LEAN", d.mean_row_terms >= 12 ? 1 : 0) != 0;
-        EvalOut eo;
-        if (eval) {
-            eo.a = eval->a; eo.b = eval->b; eo.c = eval->c;
-            eo.stride = eval->stride; eo.first = eval->first; eo.count = eval->count; eo.ab = eval->ab ? 1u : 0u;
-        }
-#define CW_LAUNCH_R1CS(PR)                                                                              \
-    do {                                                                                                \
-        if (eval) r1cs_check_kernel<PR, 3, true, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr);       \
-        else if (lean) r1cs_check_kernel<PR, 5, false, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr); \
-        else r1cs_check_kernel<PR, 3, false, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr);           \
-    } while (0)
-        if (R.prime_id == 0) CW_LAUNCH_R1CS(0);
-        else if (R.prime_id == 1) CW_LAUNCH_R1CS(1);
-        else if (eval) r1cs_check_kernel<-1, 3, true, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr);
-        else r1cs_check_kernel<-1, 3, false, false><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, nullptr);
-#undef CW_LAUNCH_R1CS
+        const EvalOut eo = eval ? *eval : EvalOut();
+        with_prime(prime_id, [&](auto pr) {
+            constexpr int PR = decltype(pr)::value;
+            if (eval) {
+                r1cs_check_kernel<PR, 3, true, false><<<g, 256, 0, stream>>>(d.general, S, fb_d, eo, nullptr);
+                return;
+            }
+            if constexpr (PR >= 0)   // (the lean build exists for bn128 and bls12381)
+                if (lean) {
+                    r1cs_check_kernel<PR, 5, false, false><<<g, 256, 0, stream>>>(d.general, S, fb_d, eo, nullptr);
+                    return;
+                }
+            r1cs_check_kernel<PR, 3, false, false><<<g, 256, 0, stream>>>(d.general, S, fb_d, eo, nullptr);
+        });
     }
     if (d.n_small) {
         // rows that are small by shape: over the integers first; the rows in which a value turned out wide (bitmap) go
         // through the general kernel afterwards
         if (!wide || eval) return fail(CW_ESTATE, "integer rows need their scratch bitmap");
         CU(cudaMemsetAsync(wide, 0, (((size_t)d.n_small + 31) / 32 + 1) * 4, stream));
-        rd.perm = d.perm_small.get();
-        rd.n_rows = d.n_small;
-        const uint64_t items = (uint64_t)d.n_small << S.bt_log2;
-        dim3 grid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
-        R1csSmallDev sg;
-        sg.groups = d.sgroups.get();
-        sg.recs = d.srecs.get();
-        sg.brow = d.sbrow.get();
-        if (S.bt_log2 == 0) r1cs_small_kernel<true><<<grid, 256, 0, stream>>>(rd, sg, S, fb_d, wide);
-        else r1cs_small_kernel<false><<<grid, 256, 0, stream>>>(rd, sg, S, fb_d, wide);
-        EvalOut eo;
-        if (R.prime_id == 0) r1cs_check_kernel<0, 3, false, true><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, wide);
-        else if (R.prime_id == 1) r1cs_check_kernel<1, 3, false, true><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, wide);
-        else r1cs_check_kernel<-1, 3, false, true><<<grid, 256, 0, stream>>>(rd, S, fb_d, eo, wide);
+        const dim3 g = grid(d.n_small);
+        if (S.bt_log2 == 0) r1cs_small_kernel<true><<<g, 256, 0, stream>>>(d.integer, d.integer_recs, S, fb_d, wide);
+        else r1cs_small_kernel<false><<<g, 256, 0, stream>>>(d.integer, d.integer_recs, S, fb_d, wide);
+        with_prime(prime_id, [&](auto pr) {
+            r1cs_check_kernel<decltype(pr)::value, 3, false, true><<<g, 256, 0, stream>>>(d.integer, S, fb_d, EvalOut(), wide);
+        });
     }
-    if (d.n_bool && !eval) {
-        const uint64_t items = (uint64_t)d.n_bool << S.bt_log2;
-        dim3 bgrid((u32)std::max<uint64_t>(1, std::min<uint64_t>((items + 255) / 256, device_sms() * 8)), std::min<u32>(n_tiles, 65535u));
-        r1cs_bool_kernel<<<bgrid, 256, 0, stream>>>(d.bool_loc.get(), d.bool_row.get(), d.n_bool, S, fb_d);
-    }
+    if (d.n_bool && !eval)
+        r1cs_bool_kernel<<<grid(d.n_bool), 256, 0, stream>>>(d.bool_loc.get(), d.bool_row.get(), d.n_bool, S, fb_d);
     CU(cudaGetLastError());
     return CW_OK;
 }
@@ -1592,7 +1555,7 @@ int cw_r1cs_eval_batch(cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, 
     const DevR1cs *d;
     int rc = get_dev_r1cs(all, b->device, b->c, d);
     if (rc) return rc;
-    R1csOut eo;
+    EvalOut eo;
     eo.a = (uint4 *)a_dev;
     eo.b = (uint4 *)b_dev;
     eo.c = (uint4 *)c_dev;
@@ -1651,10 +1614,10 @@ static int ntt_tables_for(int device, int prime_id, u32 log_n, const NttTables *
 
 static int launch_ntt_passes(const NttPass *ps, u32 np, bool dit, const NttVecs &V, const NttTables &tb, int prime_id,
                              cudaStream_t stream) {
-    void (*kern)(NttPass, NttVecs, const u32 *, const u32 *, const u32 *, u32) =
-        prime_id == 0 ? (dit ? ntt_pass_kernel<0, true> : ntt_pass_kernel<0, false>)
-        : prime_id == 1 ? (dit ? ntt_pass_kernel<1, true> : ntt_pass_kernel<1, false>)
-                        : (dit ? ntt_pass_kernel<-1, true> : ntt_pass_kernel<-1, false>);
+    using Kernel = void (*)(NttPass, NttVecs, const u32 *, const u32 *, const u32 *, u32);
+    const Kernel kern = with_prime(prime_id, [&](auto pr) -> Kernel {
+        return dit ? ntt_pass_kernel<decltype(pr)::value, true> : ntt_pass_kernel<decltype(pr)::value, false>;
+    });
     const u32 prime = (u32)prime_id;
     CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 32 << NTT_TILE_LOG));
     for (u32 k = 0; k < np; ++k) {
@@ -1680,9 +1643,7 @@ static int run_ntt(int device, int prime_id, u32 log_n, const NttVecs &V, int mo
     if (mode == NTT_MODE_COSET) {
         if ((rc = launch_ntt_passes(dit, nt, true, V, *tb, prime_id, stream))) return rc;
     } else {
-        const u32 n = 1u << log_n;
-        dim3 grid(std::max<u32>(1u, std::min<u32>((n + 255) / 256, device_sms() * 8)), std::min<u32>(V.n_vec, 65535u));
-        ntt_bitrev_kernel<<<grid, 256, 0, stream>>>(V, log_n);
+        ntt_bitrev_kernel<<<grid_for(1ull << log_n, 256, 8, V.n_vec), 256, 0, stream>>>(V, log_n);
     }
     CU(cudaGetLastError());
     return CW_OK;
@@ -1711,14 +1672,14 @@ static int quotient_on_store(cw_r1cs *r, int device, const cw_circuit *layout, c
     uint4 *A = (uint4 *)h_dev, *B = (uint4 *)scratch_dev, *Cc = B + 2 * (size_t)count * n;
     if (rows < n)
         for (uint4 *p : {A, B, Cc}) CU(cudaMemset2DAsync(p + 2 * rows, n * 32, 0, (n - rows) * 32, count, stream));
-    R1csOut eo;
+    EvalOut eo;
     eo.a = A;
     eo.b = B;
     eo.c = Cc;
     eo.stride = n;
     eo.first = first;
     eo.count = count;
-    eo.ab = true;
+    eo.ab = 1u;
     if ((rc = launch_r1cs(t, *d, S, stream, fb_d, &eo, nullptr))) return rc;
     NttVecs V;
     V.d0 = A;
@@ -1727,10 +1688,10 @@ static int quotient_on_store(cw_r1cs *r, int device, const cw_circuit *layout, c
     V.n_vec = 3 * count;
     if ((rc = run_ntt(device, r->data.prime_id, k, V, NTT_MODE_COSET, stream))) return rc;
     const size_t tot = (size_t)count * n;
-    const u32 grid = (u32)std::max<size_t>(1, std::min<size_t>((tot + 255) / 256, (size_t)device_sms() * 8));
-    if (r->data.prime_id == 0) qap_join_kernel<0><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, 0u);
-    else if (r->data.prime_id == 1) qap_join_kernel<1><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, 1u);
-    else qap_join_kernel<-1><<<grid, 256, 0, stream>>>(A, A, B, Cc, tot, (u32)r->data.prime_id);
+    const u32 prime = (u32)r->data.prime_id;
+    with_prime(r->data.prime_id, [&](auto pr) {
+        qap_join_kernel<decltype(pr)::value><<<grid_for(tot, 256, 8), 256, 0, stream>>>(A, A, B, Cc, tot, prime);
+    });
     CU(cudaGetLastError());
     return CW_OK;
 }
@@ -1928,11 +1889,10 @@ static int msm_check_pointers(int device, const uint64_t *scalars_dev, uint64_t 
 // for G1 and G2: the digits do not depend on the group.
 static int msm_sorted_digits(const MsmPlan &p, char *S, const uint64_t *scalars_dev, uint64_t stride_elems, u32 n, u32 i0,
                              u32 cn, cudaStream_t st) {
-    const u32 n_win = cn * p.W, sms = device_sms();
+    const u32 n_win = cn * p.W;
     const uint64_t N = (uint64_t)n_win * n;
     u32 *k0 = (u32 *)(S + p.keys[0]), *k1 = (u32 *)(S + p.keys[1]), *v0 = (u32 *)(S + p.vals[0]), *v1 = (u32 *)(S + p.vals[1]);
-    dim3 grid(std::max<u32>(1, std::min<u32>((n + MSM_THREADS - 1) / MSM_THREADS, sms * 8)), std::min<u32>(cn, 65535u));
-    msm_digits_kernel<<<grid, MSM_THREADS, 0, st>>>((const uint4 *)(scalars_dev + 4 * (size_t)i0 * stride_elems),
+    msm_digits_kernel<<<grid_for(n, MSM_THREADS, 8, cn), MSM_THREADS, 0, st>>>((const uint4 *)(scalars_dev + 4 * (size_t)i0 * stride_elems),
                                                     stride_elems, n, p.c, p.W, cn, k0, v0);
     size_t cub_bytes = p.cub_bytes;
     CU(cub::DeviceRadixSort::SortPairs(S + p.cub, cub_bytes, k0, k1, v0, v1, (int)N, 0, (int)(p.c + msm_seg_bits(n_win)), st));
@@ -2400,11 +2360,10 @@ int cw_fr_batch_op(int prime_id, int op, const uint64_t *a, const uint64_t *b, c
     if ((rc = dev_alloc(Rr, n * 32 + 32))) return rc;
     if ((rc = dev_alloc(err, 4))) return rc;
     CU(cudaMemset(err.get(), 0, 4));
-    u32 grid = (u32)std::min<size_t>((n + 127) / 128, device_sms() * 16);
-    if (!grid) grid = 1;
-    if (prime_id == 0) fr_batch_op_kernel<0><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), 0u);
-    else if (prime_id == 1) fr_batch_op_kernel<1><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), 1u);
-    else fr_batch_op_kernel<-1><<<grid, 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(), (u32)prime_id);
+    with_prime(prime_id, [&](auto pr) {
+        fr_batch_op_kernel<decltype(pr)::value><<<grid_for(n, 128, 16), 128>>>(op, A.get(), B.get(), C.get(), Rr.get(), n, err.get(),
+                                                                               (u32)prime_id);
+    });
     CU(cudaGetLastError());
     CU(cudaMemcpy(r, Rr.get(), n * 32, cudaMemcpyDeviceToHost));
     int herr = 0;
@@ -2429,8 +2388,9 @@ int cw_fr_mul_bench(int prime_id, size_t n, int iters, int device, float *ms) {
     u32 grid = (u32)((n + 255) / 256);
     for (int rep = 0; rep < 2; ++rep) {
         CU(cudaEventRecord(e0.get()));
-        if (prime_id == 0) fr_mul_bench_kernel<0><<<grid, 256>>>(d.get(), n, iters);
-        else fr_mul_bench_kernel<1><<<grid, 256>>>(d.get(), n, iters);
+        with_prime(prime_id, [&](auto pr) {
+            if constexpr (decltype(pr)::value >= 0) fr_mul_bench_kernel<decltype(pr)::value><<<grid, 256>>>(d.get(), n, iters);
+        });
         CU(cudaEventRecord(e1.get()));
         CU(cudaEventSynchronize(e1.get()));
     }

@@ -8,6 +8,9 @@
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
+
+#include "u256.h"
 
 #if defined(__CUDACC__)
 #define CW_HD __host__ __device__ __forceinline__
@@ -31,6 +34,31 @@ struct FrParams {
     u32 top_mask; // lboMask on the limb of the top bit (generic/fr.cpp:16)
     u32 pad;
 };
+
+// the device's parameter record of a field (host code: the kernels read it from constant memory, the CPU builds of this
+// source from the caller)
+inline FrParams make_dev_params(const FieldParams &F) {
+    FrParams p;
+    memset(&p, 0, sizeof(p));
+    auto split = [](u32 *dst, const U256 &v) {
+        for (int i = 0; i < 4; ++i) {
+            dst[2 * i] = (u32)v.v[i];
+            dst[2 * i + 1] = (u32)(v.v[i] >> 32);
+        }
+    };
+    split(p.q, F.q);
+    split(p.half, F.half);
+    split(p.r1, F.r1);
+    split(p.r2, F.r2);
+    U256 two = u256_from_u64(2), qm2;
+    u256_sub(qm2, F.q, two);
+    split(p.qm2, qm2);
+    p.np32 = F.np32;
+    p.qbits = F.qbits;
+    // lboMask of the limb that holds the top bit; fr_mask_wrap clears the limbs above it (goldilocks: limb 1, all ones)
+    p.top_mask = (F.qbits % 32 == 0) ? 0xFFFFFFFFu : ((1u << (F.qbits % 32)) - 1u);
+    return p;
+}
 
 // ---- raw 256-bit helpers -----------------------------------------------------------------------
 // On the device the 8-limb add / subtract are single carry chains (add.cc / addc.cc: 9 integer

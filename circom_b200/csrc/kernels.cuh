@@ -6,6 +6,7 @@
 #include "fr_device.cuh"
 #include "ntt.cuh"
 #include "r1cs_small.h"
+#include "tape.h"
 
 namespace cw {
 
@@ -75,8 +76,6 @@ __device__ __forceinline__ void load_const(u32 *v, const uint4 *__restrict__ con
     v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w;
     v[4] = hi.x; v[5] = hi.y; v[6] = hi.z; v[7] = hi.w;
 }
-constexpr u32 OPD_CONST = 0x80000000u, OPD_BIT = 0x20000000u, OPD_ACC = 0x10000000u, OPD_SLOT = 0x00FFFFFFu, OPD_BITPOS = 0x1FFFFFFFu;
-constexpr u32 DST_ACC_DEV = 0x00FFFFFEu;  // destination field: accumulator 0 / 1 of a fused work item (tape.h DST_ACC)
 
 // ---- the bit plane (CW_FLAG_BITPLANE) ----------------------------------------------------------------
 // Bits produced by bit runs (the outputs of Num2Bits-style decompositions: most of the witness of limb
@@ -105,18 +104,18 @@ template <bool BP>
 __device__ __forceinline__ void load_operand(u32 *v, u32 operand, const uint4 *__restrict__ tile_base,
                                              const u32 *__restrict__ plane_base, const uint4 *__restrict__ consts,
                                              u32 bt_log2, u32 li, bool half = false) {
-    if (operand & OPD_CONST) {
+    if (operand & OPERAND_CONST) {
         if (half) {
             const uint4 lo = __ldg(&consts[2 * (size_t)(operand & 0x7FFFFFFFu)]);
             v[0] = lo.x; v[1] = lo.y; v[2] = lo.z; v[3] = lo.w;
             v[4] = v[5] = v[6] = v[7] = 0;
         } else load_const(v, consts, operand & 0x7FFFFFFFu);
-    } else if (BP && (operand & OPD_BIT)) {
-        u256_set_u32(v, load_plane_bit(plane_base, operand & OPD_BITPOS, bt_log2, li));
+    } else if (BP && (operand & OPERAND_BIT)) {
+        u256_set_u32(v, load_plane_bit(plane_base, operand & OPERAND_BITPOS_MASK, bt_log2, li));
     } else if (half) {
-        load_slot_low(v, tile_base, operand & OPD_SLOT, bt_log2, li);
+        load_slot_low(v, tile_base, operand & OPERAND_SLOT_MASK, bt_log2, li);
     } else {
-        load_slot(v, tile_base, operand & OPD_SLOT, bt_log2, li);
+        load_slot(v, tile_base, operand & OPERAND_SLOT_MASK, bt_log2, li);
     }
 }
 
@@ -304,7 +303,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
             if (FUSED && k + 1 < g1) nxt = __ldg(&tp.ops[k + 1]);   // the next word of the item travels while this one executes
             const u32 opcode = opw.x & 0xFFu, dst = opw.x >> 8;
             u32 r[8];
-            if (opcode == OP_BITS && ((opw.w >> 16) & 0xFFu) <= 32u && !(opw.y & (OPD_CONST | OPD_BIT | OPD_ACC))) {
+            if (opcode == OP_BITS && ((opw.w >> 16) & 0xFFu) <= 32u && !(opw.y & (OPERAND_CONST | OPERAND_BIT | OPERAND_ACC))) {
                 // narrow bit-field of a slot value: fetch only the one or two 32-bit words that hold it
                 const u32 kk = opw.w & 0xFFFFu, m = (opw.w >> 16) & 0xFFu, run = (opw.w >> 24) + 1u;
                 const u32 wd = kk >> 5, sh = kk & 31u;
@@ -312,7 +311,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 u32 lo, hi = 0;
                 {
                     const u32 *words = reinterpret_cast<const u32 *>(base);
-                    const size_t src = (size_t)(opw.y & OPD_SLOT) << (bt_log2 + 1);
+                    const size_t src = (size_t)(opw.y & OPERAND_SLOT_MASK) << (bt_log2 + 1);
                     const u32 w1 = wd + 1u;
                     lo = words[((src + ((size_t)(wd >> 2) << bt_log2) + li) << 2) + (wd & 3u)];
                     if (two) hi = words[((src + ((size_t)(w1 >> 2) << bt_log2) + li) << 2) + (w1 & 3u)];
@@ -340,11 +339,11 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
             } else {
                 u32 a[8], b[8];
                 const bool half = opcode >= OP_NARROW_HALF;   // width-classed operators on operands below 2^128
-                if (FUSED && !(opw.y & OPD_CONST) && (opw.y & OPD_ACC)) {
+                if (FUSED && !(opw.y & OPERAND_CONST) && (opw.y & OPERAND_ACC)) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) a[i] = acc[(8 * (opw.y & 1u) + i) * blockDim.x];
                 } else load_operand<BP>(a, opw.y, base, plane_base, tp.consts, bt_log2, li, half);
-                if (FUSED && !(opw.z & OPD_CONST) && (opw.z & OPD_ACC)) {
+                if (FUSED && !(opw.z & OPERAND_CONST) && (opw.z & OPERAND_ACC)) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) b[i] = acc[(8 * (opw.z & 1u) + i) * blockDim.x];
                 } else load_operand<BP>(b, opw.z, base, plane_base, tp.consts, bt_log2, li, half);
@@ -371,7 +370,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
                 }
             }
             if (has_value) {
-                if (FUSED && dst >= DST_ACC_DEV) {
+                if (FUSED && dst >= DST_ACC) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) acc[(8 * (dst & 1u) + i) * blockDim.x] = r[i];
                 } else store_slot(r, base, dst, bt_log2, li);
@@ -433,7 +432,7 @@ __global__ void __launch_bounds__(CW_TAPE_LB, CW_TAPE_MINB)
 // ---- where the values of an instance live --------------------------------------------------------------
 // The tape's value store (tile layout, optional bit plane) or - for witnesses handed in by a caller - a dense
 // array of 32-byte rows (bt_log2 = 0, n_bitwords = 0, n_slots = row stride, location = wire id).
-// A *location* is an operand word of the tape: OPD_BIT | (word * 32 + bit), or a slot id.
+// A *location* is an operand word of the tape: OPERAND_BIT | (word * 32 + bit), or a slot id.
 struct StoreDev {
     const uint4 *slots;
     const u32 *plane;
@@ -459,8 +458,8 @@ __device__ __forceinline__ void load_slot_nc(u32 *v, const uint4 *__restrict__ t
 }
 __device__ __forceinline__ void load_loc(u32 *v, const StoreDev &S, const uint4 *__restrict__ tile_base,
                                          const u32 *__restrict__ plane_base, u32 loc, u32 li) {
-    if (loc & OPD_BIT) {
-        const u32 pos = loc & OPD_BITPOS;
+    if (loc & OPERAND_BIT) {
+        const u32 pos = loc & OPERAND_BITPOS_MASK;
         u256_set_u32(v, (__ldg(&plane_base[((size_t)(pos >> 5) << S.bt_log2) + li]) >> (pos & 31u)) & 1u);
     } else {
         load_slot_nc(v, tile_base, loc, S.bt_log2, li);
@@ -820,7 +819,7 @@ __global__ void __launch_bounds__(256, 6) r1cs_small_kernel(R1csDev R, R1csSmall
                         }
                     } else {
                         u32 x[8];
-                        load_slot_nc(x, tb, rec.x & OPD_SLOT, bt_log2, li);
+                        load_slot_nc(x, tb, rec.x & OPERAND_SLOT_MASK, bt_log2, li);
                         const u32 upper = x[1] | x[2] | x[3] | x[4] | x[5] | x[6] | x[7];
                         // the boolean constraint x*(x-1) = 0 of this wire rides on the term, as in the general kernel
                         if ((rec.x & SM_BROW) && (upper || x[0] > 1u)) atomicMin(&first_bad[inst], (unsigned long long)__ldg(&G.brow[at]));

@@ -6,31 +6,20 @@ namespace cw {
 
 cudaError_t tape_calls_set_params(const FrParams *table, size_t bytes) { return cudaMemcpyToSymbol(c_fr, table, bytes); }
 
+// every build of this unit has the function machine
 template <int PR, bool BP, int BT, bool FU>
-static void launch_k(const TapeDev &tp, uint4 *slots, u32 *plane, u32 bt_log2, u32 *first_assert, int *err, u32 batch,
-                     u32 tiles, u32 threads, cudaStream_t stream) {
-    tape_exec_kernel<PR, true, BP, BT, FU><<<tiles, threads, 0, stream>>>(tp, slots, plane, bt_log2, first_assert, err, batch);
+static bool launch_k(const TapeBuild &k, const TapeLaunch &a) {
+    return launch_tape_k<PR, true, BP, BT, FU>(k, a);
 }
 
-// warp-per-op tiles with a bit plane - the large-batch layout - get the build with the tile size fixed at compile time also
-// with calls; everything else runs the builds that take the tile size as an argument
-template <int PR>
-static void launch_pr(const TapeDev &tp, uint4 *slots, u32 *plane, u32 bt_log2, u32 *first_assert, int *err, u32 batch,
-                      u32 tiles, u32 threads, bool bp, bool fused, cudaStream_t stream) {
-#define CW_ARGS tp, slots, plane, bt_log2, first_assert, err, batch, tiles, threads, stream
-    (void)fused;   // (the lowering does not fuse tapes with calls: measured slower, flatten.cpp)
-    if (bp) {
-        if (bt_log2 == 5) launch_k<PR, true, 5, false>(CW_ARGS);
-        else launch_k<PR, true, -1, false>(CW_ARGS);
-    } else launch_k<PR, false, -1, false>(CW_ARGS);
-}
-
-void launch_tape_calls(int prime, const TapeDev &tp, uint4 *slots, u32 *plane, u32 bt_log2, u32 *first_assert, int *err,
-                       u32 batch, u32 tiles, u32 threads, bool bp, bool fused, cudaStream_t stream) {
-    if (prime == 0) launch_pr<0>(tp, slots, plane, bt_log2, first_assert, err, batch, tiles, threads, bp, fused, stream);
-    else if (prime == 1) launch_pr<1>(tp, slots, plane, bt_log2, first_assert, err, batch, tiles, threads, bp, fused, stream);
-    else launch_k<-1, true, -1, false>(CW_ARGS);   // (the lowering does not fuse for the generic-prime build)
-#undef CW_ARGS
+bool launch_tape_calls(const TapeBuild &k, const TapeLaunch &a) {
+    return with_prime(k.prime, [&](auto pr) {
+        constexpr int PR = decltype(pr)::value;
+        if constexpr (PR >= 0)
+            return launch_k<PR, true, 5, false>(k, a) || launch_k<PR, true, -1, false>(k, a) || launch_k<PR, false, -1, false>(k, a);
+        else
+            return launch_k<-1, true, -1, false>(k, a);
+    });
 }
 
 }  // namespace cw

@@ -79,6 +79,7 @@ def _load() -> ctypes.CDLL:
         "cw_batch_get_witness": (c_int, [P, c_void_p]),
         "cw_batch_last_d2h_bytes": (c_uint64, [P]),
         "cw_batch_layout": (c_int, [P, POINTER(c_uint32), POINTER(c_uint32), POINTER(c_uint64)]),
+        "cw_batch_tape_build": (c_int, [P, c_void_p]),
         "cw_batch_get_witness_async": (c_int, [P, c_void_p]),
         "cw_batch_get_witness_wait": (c_int, [P]),
         "cw_batch_get_witness_packed": (c_int, [P, c_void_p]),

@@ -381,6 +381,12 @@ class Batch:
         check(lib.cw_batch_layout(self._h, ctypes.byref(bt), ctypes.byref(th), ctypes.byref(by)))
         return bt.value, th.value, by.value
 
+    def tape_build(self):
+        """the interpreter build run() launches: (prime or -1, calls, bit plane, compile-time log2 tile size or -1, fused)"""
+        k = (ctypes.c_int32 * 5)()
+        check(lib.cw_batch_tape_build(self._h, k))
+        return k[0], bool(k[1]), bool(k[2]), k[3], bool(k[4])
+
     def expand_witness(self, first: int, count: int, device_ptr: int) -> None:
         check(lib.cw_batch_expand_witness(self._h, first, count, ctypes.c_void_p(device_ptr)))
 

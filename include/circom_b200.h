@@ -164,6 +164,11 @@ void cw_batch_destroy(cw_batch *b);
  * along the ops of a level; 5: a warp per op over 32 instances), threads per CTA, bytes of value store per instance
  * (32 * n_slots + 4 * n_bitwords).  Environment overrides: CW_BT_LOG2, CW_THREADS. */
 int cw_batch_layout(const cw_batch *b, uint32_t *bt_log2, uint32_t *threads, uint64_t *bytes_per_instance);
+/* which build of the tape interpreter cw_batch_run launches for this batch: out = {prime (0 bn128, 1 bls12381, -1: the
+ * build that takes the prime at run time), function calls, bit plane, log2 of the tile size fixed at compile time (-1: the
+ * build that takes it at run time), fused work items}.  No device work; valid before cw_batch_run.  CW_ESTATE when
+ * cw_batch_run would refuse the tape (CW_FLAG_FUSE on a prime other than bn128 / bls12381). */
+int cw_batch_tape_build(const cw_batch *b, int32_t out[5]);
 /* Circom_CalcWit::setInputSignal(h, i, val) for one instance (calcwit.cpp:77-97); host staging */
 int cw_batch_set_input(cw_batch *b, uint32_t instance, uint64_t name_hash, uint32_t idx, const uint64_t limbs[4]);
 /* getRemaingInputsToBeSet (calcwit.hpp:50-52) for one instance */

@@ -16,28 +16,6 @@
 
 using namespace cw;
 
-static FrParams dev_params(const FieldParams &F) {
-    FrParams p;
-    memset(&p, 0, sizeof(p));
-    auto split = [](u32 *dst, const U256 &v) {
-        for (int i = 0; i < 4; ++i) {
-            dst[2 * i] = (u32)v.v[i];
-            dst[2 * i + 1] = (u32)(v.v[i] >> 32);
-        }
-    };
-    split(p.q, F.q);
-    split(p.half, F.half);
-    split(p.r1, F.r1);
-    split(p.r2, F.r2);
-    U256 two = u256_from_u64(2), qm2;
-    u256_sub(qm2, F.q, two);
-    split(p.qm2, qm2);
-    p.np32 = F.np32;
-    p.qbits = F.qbits;
-    p.top_mask = (F.qbits % 32 == 0) ? 0xFFFFFFFFu : ((1u << (F.qbits % 32)) - 1u);
-    return p;
-}
-
 static std::string g_err;
 
 static unsigned long long g_narrow_calls = 0, g_wide_calls = 0;   // calls finished on the 128-bit / the full-width machine
@@ -185,7 +163,7 @@ int hs_run(const uint8_t *cb2c, size_t len, uint32_t flags, const uint64_t *inpu
         g_err = e.what();
         return -1;
     }
-    FrParams P = dev_params(t.F);
+    FrParams P = make_dev_params(t.F);
     size_t n_ops = t.n_tape_ops();
     if (stats) {
         stats[0] = t.n_signals; stats[1] = n_ops; stats[2] = t.n_levels(); stats[3] = t.n_slots;
@@ -554,7 +532,7 @@ int hs_check_levels(const uint8_t *cb2c, size_t len, uint32_t flags) {
 // single field op with the same representation handling as fr_batch_op_kernel
 int hs_fr_op(int prime, int op, const uint64_t *A, const uint64_t *B, const uint64_t *C, uint64_t *R, size_t n) {
     FieldParams F = make_field(prime);
-    FrParams P = dev_params(F);
+    FrParams P = make_dev_params(F);
     int any_err = 0;
     for (size_t i = 0; i < n; ++i) {
         u32 a[8], b[8] = {0}, c[8] = {0}, r[8];
@@ -612,7 +590,7 @@ int hs_r1cs_check(const uint8_t *cb2c, size_t len, const uint64_t *witness, uint
         g_err = e.what();
         return -1;
     }
-    FrParams P = dev_params(t.F);
+    FrParams P = make_dev_params(t.F);
     const R1csData &R = t.r1cs;
     std::vector<U256> dm(R.dict.size());
     for (size_t i = 0; i < dm.size(); ++i) dm[i] = t.F.to_mont(R.dict[i]);

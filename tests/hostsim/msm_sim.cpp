@@ -10,29 +10,8 @@
 
 using namespace cw;
 
-static FrParams dev_params(const FieldParams &F) {
-    FrParams p;
-    memset(&p, 0, sizeof(p));
-    auto split = [](u32 *dst, const U256 &v) {
-        for (int i = 0; i < 4; ++i) {
-            dst[2 * i] = (u32)v.v[i];
-            dst[2 * i + 1] = (u32)(v.v[i] >> 32);
-        }
-    };
-    split(p.q, F.q);
-    split(p.half, F.half);
-    split(p.r1, F.r1);
-    split(p.r2, F.r2);
-    U256 qm2;
-    u256_sub(qm2, F.q, u256_from_u64(2));
-    split(p.qm2, qm2);
-    p.np32 = F.np32;
-    p.qbits = F.qbits;
-    return p;
-}
-
 static const FrParams &params() {
-    static const FrParams P = dev_params(make_field(MSM_PRIME));
+    static const FrParams P = make_dev_params(make_field(MSM_PRIME));
     return P;
 }
 

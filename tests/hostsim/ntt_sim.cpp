@@ -7,27 +7,6 @@
 
 using namespace cw;
 
-static FrParams dev_params(const FieldParams &F) {
-    FrParams p;
-    memset(&p, 0, sizeof(p));
-    auto split = [](u32 *dst, const U256 &v) {
-        for (int i = 0; i < 4; ++i) {
-            dst[2 * i] = (u32)v.v[i];
-            dst[2 * i + 1] = (u32)(v.v[i] >> 32);
-        }
-    };
-    split(p.q, F.q);
-    split(p.half, F.half);
-    split(p.r1, F.r1);
-    split(p.r2, F.r2);
-    U256 qm2;
-    u256_sub(qm2, F.q, u256_from_u64(2));
-    split(p.qm2, qm2);
-    p.np32 = F.np32;
-    p.qbits = F.qbits;
-    return p;
-}
-
 static void run_passes(const NttPass *ps, u32 np, bool dit, u32 *vec, const u32 *tw, const u32 *shi, const u32 *slo,
                        const FrParams &P) {
     for (u32 k = 0; k < np; ++k) {
@@ -55,7 +34,7 @@ static void run_passes(const NttPass *ps, u32 np, bool dit, u32 *vec, const u32 
 extern "C" int ntt_sim(int prime_id, uint32_t log_n, uint32_t count, uint64_t *data, int mode) {
     const FieldParams F = make_field(prime_id);
     if (log_n < 1 || log_n + 1 > ntt_two_adicity(F)) return -1;
-    const FrParams P = dev_params(F);
+    const FrParams P = make_dev_params(F);
     std::vector<U256> tw, shi, slo;
     ntt_tables(F, log_n, tw, shi, slo);
     const u32 lg_lo = ntt_lg_lo(log_n);

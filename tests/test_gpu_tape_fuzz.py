@@ -26,10 +26,10 @@ from tests.test_lowering_fuzz_cpu import bit_logic_template, rand_input, random_
 from tests.util import ROOT, edge_values, flat_inputs, hostsim_run
 
 SEEDS = int(os.environ.get("CW_GPU_FUZZ_SEEDS", "12"))
-OP_BITS, OP_CALL = 29, 45
+OP_BITS = 29
 OPD_CONST, OPD_BIT, OPD_ACC = 0x80000000, 0x20000000, 0x10000000
 
-# One row per tape_exec_kernel<PRIME, HAS_CALLS, BP, BT, FUSED> the launchers reach (capi.cu launch_tape / cw_batch_run,
+# One row per tape_exec_kernel<PRIME, HAS_CALLS, BP, BT, FUSED> the launchers reach (capi.cu launch_tape,
 # tape_calls.cu launch_tape_calls).  kernel = (PRIME, HAS_CALLS, BP, BT, FUSED) with PRIME -1 for the run-time-indexed
 # build; bts = the tile sizes (CW_BT_LOG2) the row runs at.  Rows of the bit-plane builds use circuits that contain a bit run.
 Row = namedtuple("Row", "name prime calls compact fuse bts kernel")
@@ -56,26 +56,6 @@ BUILDS += [
 # instances per batch at each tile size: the last tile partial, at least two tiles
 BATCHES = {0: (1, 3), 2: (7,), 3: (13,), 5: (45,)}
 SMALL_THREADS = "32"   # fewer threads than the items of a level; COOP with one warp
-
-
-def dispatched_build(c, b):
-    """the kernel cw_batch_run launches for circuit c at batch b's layout (capi.cu cw_batch_run / launch_tape,
-    tape_calls.cu launch_pr), from the circuit's statistics; None: the run is refused"""
-    bt = b.layout()[0]
-    ops, _, _ = c.tape()
-    calls = bool(((ops[:, 0] & 0xFF) == OP_CALL).any())
-    bp = c.stats["n_bitwords"] != 0
-    fused = c.stats["n_items"] != c.stats["n_tape_ops"]
-    if c.prime_id not in (0, 1):
-        return None if fused else (-1, calls, True, -1, False)
-    pr = c.prime_id
-    if calls:
-        return (pr, True, bp, 5 if bp and bt == 5 else -1, False)
-    if fused:
-        return (pr, False, True, 5 if bt == 5 else -1, True)
-    if bp:
-        return (pr, False, True, bt if bt in (0, 5) else -1, False)
-    return (pr, False, False, 0 if bt == 0 else -1, False)
 
 
 def launched_builds():
@@ -187,7 +167,7 @@ def _check_row_runs(monkeypatch, row, d, ins, exps, tag):
                 assert n <= n_max
                 for th in (None, SMALL_THREADS):
                     b = _run(monkeypatch, c, d, ins[:n], bt, th)
-                    assert dispatched_build(c, b) == row.kernel, (tag, bt)
+                    assert b.tape_build() == row.kernel, (tag, bt)
                     st = b.status()
                     assert not st.any(), (tag, flags, bt, n, th, st)
                     wit = b.witness()
@@ -220,9 +200,10 @@ def test_random_templates_on_every_build(row, monkeypatch):
             assert c.stats["n_items"] < c.stats["n_tape_ops"]
             b = Batch(c, len(ins))
             b.set_inputs(flat_inputs(d, ins))
-            with pytest.raises(CwError) as e:
-                b.run()
-            assert e.value.code == native.CW_ESTATE
+            for refused in (b.tape_build, b.run):
+                with pytest.raises(CwError) as e:
+                    refused()
+                assert e.value.code == native.CW_ESTATE
     assert ran >= (SEEDS + 1) // 2, ran
 
 
@@ -263,7 +244,7 @@ def test_random_function_bodies_on_the_call_builds(name, prime, bt, compact, ker
         want = _expected(exps, w2s)
         for th in (None, SMALL_THREADS):
             b = _run(monkeypatch, c, d, ins, bt, th)
-            assert dispatched_build(c, b) == kernel
+            assert b.tape_build() == kernel
             assert not b.status().any(), (name, seed, b.status())
             wit = b.witness()
             assert (wit == want).all(), "%s seed %d threads %s: (instance, entry) %s differ" % (name, seed, th, _diff(wit, want))
@@ -353,7 +334,7 @@ def test_bit_field_fetch_sweep(prime, monkeypatch):
         want = E[:, w2s]
         for th in (None, SMALL_THREADS):
             b = _run(monkeypatch, c, d, ins, bt, th)
-            assert dispatched_build(c, b) == (c.prime_id,) + kernel, name
+            assert b.tape_build() == (c.prime_id,) + kernel, name
             assert not b.status().any()
             wit = b.witness()
             if not (wit == want).all():
