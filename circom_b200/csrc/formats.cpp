@@ -176,6 +176,8 @@ void read_r1cs(const std::string &path, R1csData &out) {
             if (it == idx.end()) {
                 U256 c = u256_from_u64(0);
                 memcpy(c.v, key.data(), fs);
+                // the check's arithmetic takes canonical coefficients (kinds by exact comparison with 2^k and q - 2^k)
+                if (!(c < q)) throw std::runtime_error("r1cs: coefficient not reduced modulo the prime");
                 id = (uint32_t)out.dict.size();
                 out.dict.push_back(c);
                 idx.emplace(std::move(key), id);

@@ -57,7 +57,8 @@ void compile_r1cs_host(const R1csData &R, const FieldParams &F, const Tape *T, b
         uint64_t p0 = R.row_ptr[3 * row], p1 = R.row_ptr[3 * row + 1], p2 = R.row_ptr[3 * row + 2], p3 = R.row_ptr[3 * row + 3];
         bool is_bool = false;
         u32 wire = 0;
-        if (p3 == p2 && (p1 - p0) + (p2 - p1) == 3) {
+        // (one block of one term, the other of two: three terms in A with B and C empty is A * 0 = 0, no boolean row)
+        if (p3 == p2 && ((p1 - p0 == 1 && p2 - p1 == 2) || (p1 - p0 == 2 && p2 - p1 == 1))) {
             uint64_t s0 = (p1 - p0 == 1) ? p0 : p1, l0 = (p1 - p0 == 1) ? p1 : p0;  // single-term block / two-term block
             // two-term block is sorted by wire: {one: -1, x: +1}
             if (is_unit(s0, 1) && R.col[s0] != 0 && R.col[l0] == 0 && is_unit(l0, 2) && R.col[l0 + 1] == R.col[s0] && is_unit(l0 + 1, 1)) {

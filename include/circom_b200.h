@@ -242,7 +242,8 @@ int cw_batch_wtns_bytes(cw_batch *b, uint32_t instance, uint8_t *out, size_t cap
 /* ---- R1CS --------------------------------------------------------------------------------- */
 /* constraints of the loaded circuit in witness numbering */
 int cw_r1cs_from_circuit(const cw_circuit *c, cw_r1cs **out);
-/* parse a .r1cs file (layout of constraint_writers/src/r1cs_writer.rs:93-101,49-72,246-269,328-341) */
+/* parse a .r1cs file (layout of constraint_writers/src/r1cs_writer.rs:93-101,49-72,246-269,328-341); a coefficient not
+ * reduced modulo the prime is CW_EFORMAT */
 int cw_r1cs_load(const char *path, cw_r1cs **out);
 /* write it back in the reference's section order (constraint_list/src/r1cs_porting.rs:19-53); a count given as
  * CW_KEEP keeps the value the circuit / the loaded file carries */

@@ -619,6 +619,33 @@ int hs_r1cs_check(const uint8_t *cb2c, size_t len, const uint64_t *witness, uint
     return 0;
 }
 
+// Census of the general-row terms the R1CS check compiles for the value layout of the lowered tape (r1cs_compile.cpp):
+// out[0] runs of plane bits, out[1] runs at a shift above 80 (placed without the lazy 128-bit sum), out[2] runs with a
+// negative coefficient, out[3] runs that start inside a plane word, out[4] runs of 32 bits at shift 96, out[5] terms
+int hs_r1cs_term_census(const uint8_t *cb2c, size_t len, uint32_t flags, uint64_t *out) {
+    Tape t;
+    R1csCompiled C;
+    try {
+        lower_circuit(cb2c, len, flags, t);
+        compile_r1cs_host(t.r1cs, t.F, &t, false, false, C);
+    } catch (const std::exception &e) {
+        g_err = e.what();
+        return -1;
+    }
+    for (int i = 0; i < 6; ++i) out[i] = 0;
+    for (const R1csTerm &tm : C.terms) {
+        const u32 kd = tm.kind & 0xFFu, sh = (tm.kind >> 8) & 0xFFu, first = (tm.kind >> 16) & 31u, cnt = ((tm.kind >> 21) & 31u) + 1u;
+        if (kd < 5u) continue;
+        out[0] += 1;
+        out[1] += sh > 80u;
+        out[2] += kd == 6u;
+        out[3] += first != 0u;
+        out[4] += sh == 96u && cnt == 32u;
+    }
+    out[5] = C.terms.size();
+    return 0;
+}
+
 int hs_write_r1cs(const uint8_t *cb2c, size_t len, const char *path) {
     Tape t;
     try {
