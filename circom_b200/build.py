@@ -8,15 +8,16 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcircom_b200.so")
 CLI = os.path.join(HERE, "circom_cuda_witness")
-SOURCES = ["capi.cu", "tape_calls.cu", "msm_g2.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
-CLI_SOURCES = ["cli.cpp"]
-HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "msm_g2.cuh", "msm_g2.h", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
+PROVER = os.path.join(HERE, "circom_cuda_prover")
+SOURCES = ["capi.cu", "tape_calls.cu", "msm_g2.cu", "groth16.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
+CLI_SOURCES = ["cli.cpp", "prover_cli.cpp"]
+HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "msm_g2.cuh", "msm_g2.h", "groth16.cuh", "groth16.h", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 
 
 def _stale() -> bool:
-    if not os.path.exists(LIB) or not os.path.exists(CLI):
+    if not os.path.exists(LIB) or not os.path.exists(CLI) or not os.path.exists(PROVER):
         return True
     t = os.path.getmtime(LIB)
     return any(os.path.getmtime(os.path.join(CSRC, f)) > t for f in SOURCES + HEADERS + CLI_SOURCES)
@@ -43,6 +44,14 @@ def build(force: bool = False, verbose: bool = False) -> str:
                         "-lcircom_b200", "-Wl,-rpath,$ORIGIN"], capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("g++ (cli) failed:\n" + r.stderr[-4000:])
+    # command-line prover (client of the C ABI; its device buffers come from the CUDA runtime)
+    cuda = os.path.dirname(os.path.dirname(os.path.realpath(nvcc)))
+    r = subprocess.run(["g++", "-O2", "-std=c++17", "-o", PROVER, os.path.join(CSRC, "prover_cli.cpp"),
+                        "-I" + os.path.join(cuda, "include"), "-L" + HERE, "-lcircom_b200", "-Wl,-rpath,$ORIGIN",
+                        "-L" + os.path.join(cuda, "lib64"), "-lcudart_static", "-ldl", "-lrt", "-lpthread"],
+                       capture_output=True, text=True)
+    if r.returncode != 0:
+        raise RuntimeError("g++ (prover) failed:\n" + r.stderr[-4000:])
     return LIB
 
 

@@ -20,6 +20,8 @@
 #include <mutex>
 #include <thread>
 #include <stdexcept>
+#include <cerrno>
+#include <sys/random.h>
 #include <string>
 #include <vector>
 
@@ -29,6 +31,7 @@
 #include "kernels.cuh"
 #include "msm.cuh"
 #include "msm_g2.h"
+#include "groth16.h"
 #include "tape_calls.h"
 #include "tape.h"
 #include "hostpack.h"
@@ -114,6 +117,7 @@ int ensure_device(int device) {
         CU(cudaMemcpyToSymbol(c_fr, h, sizeof(h)));
         CU(tape_calls_set_params(h, sizeof(h)));
         CU(msm_g2_set_params(h, sizeof(h)));
+        CU(groth16_set_params(h, sizeof(h)));
         g_dev_ready[device] = true;
     }
     return CW_OK;
@@ -216,6 +220,7 @@ struct cw_r1cs {
     std::map<R1csKey, DevR1cs> dev;
     std::unique_ptr<cw_r1cs> eval_twin;  // the same constraints compiled without boolean-row special cases (cw_r1cs_eval_batch)
     std::unique_ptr<cw_r1cs> qap_twin;   // ... plus the rows a_{m+j} = w_j, j <= nPublic (cw_r1cs_quotient_*)
+    uint64_t digest = 0;                 // content hash of the constraints (r1cs_digest; 0: not computed yet)
     bool no_bool_rows = false;
 };
 
@@ -1813,36 +1818,53 @@ static int msm_plan_for(uint64_t n, u32 count, MsmPlan &p, size_t pt_bytes = siz
     return msm_plan(n, (u32)chunk, p, pt_bytes);
 }
 
-int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g1_bases **out) {
-    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
-    *out = nullptr;
-    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G1 bases are built for bn128 (BN254) only");
-    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+// n affine G1 points [n][2][4] u64 - canonical, or Montgomery images when `mont` (as a .zkey stores them) - checked on
+// the host: (0, 0) is infinity, anything else has both coordinates below q and lies on the curve; out receives the
+// Montgomery images the MSM reads.  `what` prefixes the messages, which name the first bad index.
+static int g1_points_mont(const uint64_t *points, uint64_t n, bool mont, const std::string &what, std::vector<U256> &out) {
     const FieldParams F = make_field(MSM_PRIME);
     const U256 three = F.to_mont(u256_from_u64(3));
-    std::vector<U256> mont(2 * n);
+    out.assign(2 * n, U256());
     for (uint64_t i = 0; i < n; ++i) {
         U256 x, y;
         memcpy(x.v, points + 8 * i, 32);
         memcpy(y.v, points + 8 * i + 4, 32);
         if (x.is_zero() && y.is_zero()) {
-            mont[2 * i] = x;
-            mont[2 * i + 1] = y;
+            out[2 * i] = x;
+            out[2 * i + 1] = y;
             continue;
         }
-        if (!(x < F.q) || !(y < F.q)) return fail(CW_EINVAL, "point " + std::to_string(i) + ": a coordinate is not below q");
-        const U256 xm = F.to_mont(x), ym = F.to_mont(y);
+        if (!(x < F.q) || !(y < F.q)) return fail(CW_EINVAL, what + "point " + std::to_string(i) + ": a coordinate is not below q");
+        const U256 xm = mont ? x : F.to_mont(x), ym = mont ? y : F.to_mont(y);
         if (F.mont_mul(ym, ym) != F.addm(F.mont_mul(F.mont_mul(xm, xm), xm), three))
-            return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the curve y^2 = x^3 + 3");
-        mont[2 * i] = xm;
-        mont[2 * i + 1] = ym;
+            return fail(CW_EINVAL, what + "point " + std::to_string(i) + " is not on the curve y^2 = x^3 + 3");
+        out[2 * i] = xm;
+        out[2 * i + 1] = ym;
     }
+    return CW_OK;
+}
+// checked Montgomery images (g1_points_mont) to a new handle on `device`
+static int g1_bases_upload(const std::vector<U256> &mont, int device, std::unique_ptr<cw_g1_bases> &out) {
     int rc = ensure_device(device);
     if (rc) return rc;
     auto b = std::make_unique<cw_g1_bases>();
     b->device = device;
-    b->n = n;
-    if ((rc = upload(b->pts, mont.data(), (size_t)n * 64))) return rc;
+    b->n = mont.size() / 2;
+    if ((rc = upload(b->pts, mont.data(), (size_t)b->n * 64))) return rc;
+    out = std::move(b);
+    return CW_OK;
+}
+
+int cw_g1_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g1_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G1 bases are built for bn128 (BN254) only");
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    std::vector<U256> mont;
+    int rc = g1_points_mont(points, n, false, "", mont);
+    if (rc) return rc;
+    std::unique_ptr<cw_g1_bases> b;
+    if ((rc = g1_bases_upload(mont, device, b))) return rc;
     *out = b.release();
     return CW_OK;
 }
@@ -1956,11 +1978,9 @@ static const uint64_t G2_TWIST_B[2][4] = {
     {0xe4a2bd0685c315d2ull, 0xa74fa084e52d1852ull, 0xcd2cafadeed8fdf4ull, 0x009713b03af0fed4ull},
 };
 
-int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g2_bases **out) {
-    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
-    *out = nullptr;
-    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G2 bases are built for bn128 (BN254) only");
-    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+// n affine G2 points [n][2][2][4] u64, canonical or Montgomery images (`mont`), checked as g1_points_mont does: all zeros
+// is infinity, anything else has its four coefficients below q and lies on E'
+static int g2_points_mont(const uint64_t *points, uint64_t n, bool mont, const std::string &what, std::vector<U256> &out) {
     const FieldParams F = make_field(MSM_PRIME);
     // Fq2 on the host, Montgomery images (c0, c1): the check y^2 = x^3 + b' is written apart from the device formulas
     struct E2 { U256 c0, c1; };
@@ -1973,7 +1993,7 @@ int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int dev
     memcpy(b0.v, G2_TWIST_B[0], 32);
     memcpy(b1.v, G2_TWIST_B[1], 32);
     const E2 bt{F.to_mont(b0), F.to_mont(b1)};
-    std::vector<U256> mont(4 * n);
+    out.assign(4 * n, U256());
     for (uint64_t i = 0; i < n; ++i) {
         U256 c[4];
         bool zero = true;
@@ -1982,28 +2002,43 @@ int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int dev
             zero = zero && c[k].is_zero();
         }
         if (zero) {
-            for (int k = 0; k < 4; ++k) mont[4 * i + k] = c[k];
+            for (int k = 0; k < 4; ++k) out[4 * i + k] = c[k];
             continue;
         }
         for (int k = 0; k < 4; ++k)
             if (!(c[k] < F.q))
-                return fail(CW_EINVAL, "point " + std::to_string(i) + ": coefficient " + std::to_string(k) +
+                return fail(CW_EINVAL, what + "point " + std::to_string(i) + ": coefficient " + std::to_string(k) +
                                            " (x.c0, x.c1, y.c0, y.c1) is not below q");
-        const E2 x{F.to_mont(c[0]), F.to_mont(c[1])}, y{F.to_mont(c[2]), F.to_mont(c[3])};
+        for (int k = 0; k < 4 && !mont; ++k) c[k] = F.to_mont(c[k]);
+        const E2 x{c[0], c[1]}, y{c[2], c[3]};
         const E2 yy = mul(y, y), xxx = mul(mul(x, x), x);
         if (yy.c0 != F.addm(xxx.c0, bt.c0) || yy.c1 != F.addm(xxx.c1, bt.c1))
-            return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the twist y^2 = x^3 + 3 / (9 + u)");
-        mont[4 * i] = x.c0;
-        mont[4 * i + 1] = x.c1;
-        mont[4 * i + 2] = y.c0;
-        mont[4 * i + 3] = y.c1;
+            return fail(CW_EINVAL, what + "point " + std::to_string(i) + " is not on the twist y^2 = x^3 + 3 / (9 + u)");
+        for (int k = 0; k < 4; ++k) out[4 * i + k] = c[k];
     }
+    return CW_OK;
+}
+static int g2_bases_upload(const std::vector<U256> &mont, int device, std::unique_ptr<cw_g2_bases> &out) {
     int rc = ensure_device(device);
     if (rc) return rc;
     auto b = std::make_unique<cw_g2_bases>();
     b->device = device;
-    b->n = n;
-    if ((rc = upload(b->pts, mont.data(), (size_t)n * 128))) return rc;
+    b->n = mont.size() / 4;
+    if ((rc = upload(b->pts, mont.data(), (size_t)b->n * 128))) return rc;
+    out = std::move(b);
+    return CW_OK;
+}
+
+int cw_g2_bases_create(int prime_id, const uint64_t *points, uint64_t n, int device, cw_g2_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "G2 bases are built for bn128 (BN254) only");
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    std::vector<U256> mont;
+    int rc = g2_points_mont(points, n, false, "", mont);
+    if (rc) return rc;
+    std::unique_ptr<cw_g2_bases> b;
+    if ((rc = g2_bases_upload(mont, device, b))) return rc;
     *out = b.release();
     return CW_OK;
 }
@@ -2058,6 +2093,421 @@ int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride
         CU(cudaGetLastError());
     }
     return CW_OK;
+}
+
+// ---- Groth16 proofs: proving key (.zkey), prove calls, assembly (groth16.cuh, kernel in groth16.cu) -------------------
+static const int G16_STAGES = 8;   // expansion, quotient, H, A, B1, B2, C, assembly
+
+struct cw_groth16_key {
+    int device = 0;
+    uint64_t n_vars = 0, n_public = 0, log_n = 0, n_coefs = 0;
+    uint64_t r1cs_digest = 0;                     // r1cs_digest of the R1CS the key was checked against
+    std::unique_ptr<cw_g1_bases> A, B1, C, H;     // C: null when the circuit has no private signals (its term is infinity)
+    std::unique_ptr<cw_g2_bases> B2;
+    DevPtr<u32> consts;                           // Groth16Consts: alpha1, beta1, delta1, beta2, delta2 (Montgomery)
+    std::vector<uint64_t> ic;                     // [n_public + 1][2][4] canonical: the verifier's IC points
+    Event ev[G16_STAGES + 1];                     // stage boundaries of the last prove call (cw_groth16_last_ms)
+    bool timed = false;
+};
+
+// stage boundaries: recorded on the prove call's stream, read by cw_groth16_last_ms
+static int groth16_mark(cw_groth16_key *k, int stage, cudaStream_t st) {
+    if (!k->ev[stage]) {
+        int rc = make_event(k->ev[stage]);
+        if (rc) return rc;
+    }
+    CU(cudaEventRecord(k->ev[stage].get(), st));
+    return CW_OK;
+}
+
+// FNV-1a style hash over the words of the constraints (sizes, public counts, rows, wires, coefficient values): the
+// identity a proving key is tied to.  Two loads of the same .r1cs have the same digest.
+static uint64_t r1cs_digest(cw_r1cs *r) {
+    std::lock_guard<std::mutex> lk(r->mu);
+    if (r->digest) return r->digest;
+    const R1csData &R = r->data;
+    uint64_t h = 0xcbf29ce484222325ull;
+    auto mix = [&](uint64_t w) { h = (h ^ w) * 0x100000001b3ull; };
+    for (uint64_t w : {(uint64_t)R.prime_id, R.n_wires, R.n_constraints, (uint64_t)R.n_pub_out, (uint64_t)R.n_pub_in}) mix(w);
+    for (uint64_t p : R.row_ptr) mix(p);
+    for (size_t i = 0; i < R.col.size(); ++i) {
+        mix(R.col[i]);
+        for (int k = 0; k < 4; ++k) mix(R.dict[R.coef[i]].v[k]);
+    }
+    r->digest = h ? h : 1;
+    return r->digest;
+}
+
+// grumpkin = BN254's base field q, bn128 = its scalar field r: the 32-byte fields section 2 of a BN254 .zkey carries
+static const int ZKEY_Q_PRIME = CW_PRIME_GRUMPKIN, ZKEY_R_PRIME = CW_PRIME_BN128;
+
+// the .zkey bytes, checked against the R1CS on the host; pointers into the caller's buffer
+struct ZkeyView {
+    const uint8_t *sec[10] = {};   // payload of sections 1..9 (index = id)
+    uint64_t size[10] = {};
+    uint32_t n_vars = 0, n_public = 0, domain = 0, n_coefs = 0;
+};
+
+static uint32_t le32(const uint8_t *p) { uint32_t v; memcpy(&v, p, 4); return v; }
+static uint64_t le64(const uint8_t *p) { uint64_t v; memcpy(&v, p, 8); return v; }
+
+static int zkey_parse(const uint8_t *z, size_t len, cw_r1cs *r, ZkeyView &v) {
+    static const char *names[10] = {"", "header", "Groth16 header", "IC", "coefficients", "A", "B1", "B2", "C", "H"};
+    auto sec = [&](int id) { return "section " + std::to_string(id) + " (" + names[id] + ")"; };
+    if (len < 12 || memcmp(z, "zkey", 4) != 0) return fail(CW_EINVAL, "zkey: bad magic (not a .zkey file)");
+    if (le32(z + 4) != 1) return fail(CW_EINVAL, "zkey: version " + std::to_string(le32(z + 4)) + ", expected 1");
+    const uint32_t n_sections = le32(z + 8);
+    uint64_t at = 12;
+    for (uint32_t k = 0; k < n_sections; ++k) {
+        if (len - at < 12) return fail(CW_EINVAL, "zkey: truncated: the header of section record " + std::to_string(k) + " lies past the end");
+        const uint32_t id = le32(z + at);
+        const uint64_t size = le64(z + at + 4);
+        at += 12;
+        if (size > len - at)
+            return fail(CW_EINVAL, "zkey: truncated: section " + std::to_string(id) + " declares " + std::to_string(size) +
+                                       " bytes, " + std::to_string(len - at) + " remain");
+        if (id >= 1 && id <= 9) {
+            if (v.sec[id]) return fail(CW_EINVAL, "zkey: duplicate " + sec((int)id));
+            v.sec[id] = z + at;
+            v.size[id] = size;
+        }
+        at += size;   // (section 10, the contributions, and unknown sections are skipped)
+    }
+    if (at != len) return fail(CW_EINVAL, "zkey: " + std::to_string(len - at) + " bytes after the last section");
+    for (int id = 1; id <= 9; ++id)
+        if (!v.sec[id]) return fail(CW_EINVAL, "zkey: missing " + sec(id));
+    if (v.size[1] != 4) return fail(CW_EINVAL, "zkey: " + sec(1) + " has " + std::to_string(v.size[1]) + " bytes, expected 4");
+    if (le32(v.sec[1]) != 1) return fail(CW_EINVAL, "zkey: protocol " + std::to_string(le32(v.sec[1])) + " is not Groth16 (1)");
+    // section 2: n8q, q, n8r, r, nVars, nPublic, domainSize, alpha1, beta1, beta2, gamma2, delta1, delta2
+    const uint8_t *h = v.sec[2];
+    if (v.size[2] < 4) return fail(CW_EINVAL, "zkey: " + sec(2) + " is truncated");
+    const uint32_t n8q = le32(h);
+    if (n8q != 32) return fail(CW_EINVAL, "zkey: n8q = " + std::to_string(n8q) + ": only BN254 keys (32-byte fields) are read");
+    const uint64_t h_size = 4 + 32 + 4 + 32 + 12 + 3 * 64 + 3 * 128;
+    if (v.size[2] < 40) return fail(CW_EINVAL, "zkey: " + sec(2) + " is truncated");
+    const uint32_t n8r = le32(h + 36);
+    if (n8r != 32) return fail(CW_EINVAL, "zkey: n8r = " + std::to_string(n8r) + ": only BN254 keys (32-byte fields) are read");
+    if (v.size[2] != h_size)
+        return fail(CW_EINVAL, "zkey: " + sec(2) + " has " + std::to_string(v.size[2]) + " bytes, expected " + std::to_string(h_size));
+    if (memcmp(h + 4, make_field(ZKEY_Q_PRIME).q.v, 32) != 0) return fail(CW_EINVAL, "zkey: q is not the BN254 base field");
+    if (memcmp(h + 40, make_field(ZKEY_R_PRIME).q.v, 32) != 0) return fail(CW_EINVAL, "zkey: r is not the BN254 scalar field (bn128)");
+    v.n_vars = le32(h + 72);
+    v.n_public = le32(h + 76);
+    v.domain = le32(h + 80);
+    if (v.n_public >= v.n_vars)
+        return fail(CW_EINVAL, "zkey: nPublic (" + std::to_string(v.n_public) + ") must be below nVars (" + std::to_string(v.n_vars) + ")");
+    if (v.domain == 0 || (v.domain & (v.domain - 1)))
+        return fail(CW_EINVAL, "zkey: domainSize " + std::to_string(v.domain) + " is not a power of two");
+    if (v.size[4] < 4) return fail(CW_EINVAL, "zkey: " + sec(4) + " is truncated");
+    v.n_coefs = le32(v.sec[4]);
+    // the sizes the header implies, in 64-bit arithmetic (no count can wrap them)
+    const uint64_t nv = v.n_vars, np = v.n_public;
+    const uint64_t want[10] = {0, 4, h_size, (np + 1) * 64, 4 + (uint64_t)v.n_coefs * 44, nv * 64, nv * 64, nv * 128,
+                               (nv - np - 1) * 64, (uint64_t)v.domain * 64};
+    for (int id = 3; id <= 9; ++id)
+        if (v.size[id] != want[id])
+            return fail(CW_EINVAL, "zkey: " + sec(id) + " has " + std::to_string(v.size[id]) + " bytes, the header implies " +
+                                       std::to_string(want[id]));
+    // the key against the R1CS
+    const R1csData &R = r->data;
+    if (R.prime_id != CW_PRIME_BN128) return fail(CW_EINVAL, "zkey: the R1CS is not over bn128");
+    if (nv != R.n_wires)
+        return fail(CW_EINVAL, "zkey: nVars (" + std::to_string(nv) + ") differs from the R1CS's wires (" + std::to_string(R.n_wires) + ")");
+    u32 log_n = 0, n_pub = 0;
+    int rc = qap_domain(r, log_n, n_pub);
+    if (rc) return rc;
+    if (np != n_pub)
+        return fail(CW_EINVAL, "zkey: nPublic (" + std::to_string(np) + ") differs from the R1CS's (" + std::to_string(n_pub) + ")");
+    if ((uint64_t)v.domain != (1ull << log_n))
+        return fail(CW_EINVAL, "zkey: domainSize " + std::to_string(v.domain) + " disagrees with the R1CS's domain 2^" + std::to_string(log_n));
+    // section 4 as a multiset of (matrix, constraint, signal): the nonzero A and B terms of the R1CS and the rows
+    // A[m + j][j] = 1, j <= nPublic.  The coefficient values are not compared: which form snarkjs stores them in (they
+    // are scaled Montgomery images there) could not be confirmed against a file snarkjs wrote, and the quotient reads
+    // A and B from the R1CS, so only the shape has to match.
+    using Term = std::tuple<u32, uint64_t, u32>;
+    std::vector<Term> want_t, got_t;
+    const uint64_t m = R.n_constraints;
+    for (uint64_t i = 0; i < m; ++i)
+        for (u32 mat = 0; mat < 2; ++mat)
+            for (uint64_t t = R.row_ptr[3 * i + mat]; t < R.row_ptr[3 * i + mat + 1]; ++t)
+                if (!R.dict[R.coef[t]].is_zero()) want_t.emplace_back(mat, i, R.col[t]);
+    for (uint64_t j = 0; j <= np; ++j) want_t.emplace_back(0u, m + j, (u32)j);
+    got_t.reserve(v.n_coefs);
+    for (uint64_t k = 0; k < v.n_coefs; ++k) {
+        const uint8_t *e = v.sec[4] + 4 + 44 * k;
+        got_t.emplace_back(le32(e), (uint64_t)le32(e + 4), le32(e + 8));
+    }
+    std::sort(want_t.begin(), want_t.end());
+    std::sort(got_t.begin(), got_t.end());
+    if (want_t != got_t)
+        return fail(CW_EINVAL, "zkey: " + sec(4) + " lists " + std::to_string(got_t.size()) + " (matrix, constraint, signal) terms "
+                               "that are not the R1CS's A and B terms (" + std::to_string(want_t.size()) + "): a key of another circuit");
+    return CW_OK;
+}
+
+// cw_groth16_key_info / the handle: see include/circom_b200.h
+int cw_groth16_key_create(const void *zkey, size_t len, const cw_r1cs *r_in, int device, cw_groth16_key **out) {
+    if (!out || !zkey || !r_in) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    cw_r1cs *r = const_cast<cw_r1cs *>(r_in);   // (the digest is cached in the handle)
+    ZkeyView v;
+    int rc = zkey_parse((const uint8_t *)zkey, len, r, v);
+    if (rc) return rc;
+    const uint64_t nv = v.n_vars, np = v.n_public;
+    if (nv > MSM_MAX_N || v.domain > MSM_MAX_N) return fail(CW_EINVAL, "zkey: more than 2^26 points in a base set");
+    // every point on the host before any device is touched
+    const uint8_t *h = v.sec[2] + 84;   // alpha1 +0, beta1 +64, beta2 +128, gamma2 +256, delta1 +384, delta2 +448
+    std::vector<U256> g1c, g2c, ic, a, b1, c, hh, b2;
+    std::vector<uint64_t> buf(3 * 8);
+    memcpy(buf.data(), h, 64);              // alpha1
+    memcpy(buf.data() + 8, h + 64, 64);     // beta1
+    memcpy(buf.data() + 16, h + 384, 64);   // delta1
+    if ((rc = g1_points_mont(buf.data(), 3, true, "zkey: section 2 (alpha1, beta1, delta1): ", g1c))) return rc;
+    buf.assign(3 * 16, 0);
+    memcpy(buf.data(), h + 128, 128);       // beta2
+    memcpy(buf.data() + 16, h + 256, 128);  // gamma2 (checked; the prover does not use it)
+    memcpy(buf.data() + 32, h + 448, 128);  // delta2
+    if ((rc = g2_points_mont(buf.data(), 3, true, "zkey: section 2 (beta2, gamma2, delta2): ", g2c))) return rc;
+    auto words = [](const uint8_t *p, uint64_t n_u64) {
+        std::vector<uint64_t> w(n_u64);
+        memcpy(w.data(), p, n_u64 * 8);
+        return w;
+    };
+    if ((rc = g1_points_mont(words(v.sec[3], (np + 1) * 8).data(), np + 1, true, "zkey: section 3 (IC): ", ic))) return rc;
+    if ((rc = g1_points_mont(words(v.sec[5], nv * 8).data(), nv, true, "zkey: section 5 (A): ", a))) return rc;
+    if ((rc = g1_points_mont(words(v.sec[6], nv * 8).data(), nv, true, "zkey: section 6 (B1): ", b1))) return rc;
+    if ((rc = g2_points_mont(words(v.sec[7], nv * 16).data(), nv, true, "zkey: section 7 (B2): ", b2))) return rc;
+    if ((rc = g1_points_mont(words(v.sec[8], (nv - np - 1) * 8).data(), nv - np - 1, true, "zkey: section 8 (C): ", c))) return rc;
+    if ((rc = g1_points_mont(words(v.sec[9], (uint64_t)v.domain * 8).data(), v.domain, true, "zkey: section 9 (H): ", hh))) return rc;
+    auto k = std::make_unique<cw_groth16_key>();
+    k->device = device;
+    k->n_vars = nv;
+    k->n_public = np;
+    k->n_coefs = v.n_coefs;
+    while ((1ull << k->log_n) < v.domain) ++k->log_n;
+    k->r1cs_digest = r1cs_digest(r);
+    const FieldParams F = make_field(MSM_PRIME);
+    k->ic.resize(ic.size() * 4);
+    for (size_t i = 0; i < ic.size(); ++i) {
+        const U256 cv = ic[i].is_zero() ? ic[i] : F.from_mont(ic[i]);   // ((0, 0) stays (0, 0): from_mont(0) = 0)
+        memcpy(k->ic.data() + 4 * i, cv.v, 32);
+    }
+    std::vector<U256> cs;   // Groth16Consts order: alpha1, beta1, delta1, beta2, delta2
+    cs.insert(cs.end(), g1c.begin(), g1c.end());
+    cs.insert(cs.end(), g2c.begin(), g2c.begin() + 4);
+    cs.insert(cs.end(), g2c.begin() + 8, g2c.end());
+    static_assert(G16_CONSTS_WORDS == 14 * 8, "Groth16Consts layout: 3 G1 and 2 G2 points");
+    if ((rc = g1_bases_upload(a, device, k->A))) return rc;   // (the first device call: ensure_device)
+    if ((rc = g1_bases_upload(b1, device, k->B1))) return rc;
+    if (nv - np - 1 && (rc = g1_bases_upload(c, device, k->C))) return rc;
+    if ((rc = g1_bases_upload(hh, device, k->H))) return rc;
+    if ((rc = g2_bases_upload(b2, device, k->B2))) return rc;
+    if ((rc = upload(k->consts, cs.data(), cs.size() * 32))) return rc;
+    *out = k.release();
+    return CW_OK;
+}
+
+void cw_groth16_key_destroy(cw_groth16_key *k) {
+    if (!k) return;
+    cudaSetDevice(k->device);
+    delete k;
+}
+
+int cw_groth16_key_info(const cw_groth16_key *k, uint64_t info[4]) {
+    if (!k || !info) return fail(CW_EINVAL, "null argument");
+    info[0] = k->n_vars;
+    info[1] = k->n_public;
+    info[2] = k->log_n;
+    info[3] = k->n_coefs;
+    return CW_OK;
+}
+
+int cw_groth16_key_ic(const cw_groth16_key *k, uint64_t *out) {
+    if (!k || !out) return fail(CW_EINVAL, "null argument");
+    memcpy(out, k->ic.data(), k->ic.size() * 8);
+    return CW_OK;
+}
+
+// the caller's scratch: witness rows (cw_groth16_prove_batch only), h, the MSM results, (r, s), then one work area that
+// the quotient uses first and every MSM after it (they run later on the same stream)
+struct G16Layout {
+    size_t rows = 0, h = 0, ma = 0, mb1 = 0, mc = 0, mh = 0, mb2 = 0, rs = 0, work = 0, total = 0;
+};
+static int groth16_layout(const cw_groth16_key *k, u32 count, G16Layout &L) {
+    size_t at = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = at;
+        at += (bytes + 255) & ~(size_t)255;
+        return o;
+    };
+    const size_t n = (size_t)1 << k->log_n;
+    L.rows = take((size_t)count * k->n_vars * 32);
+    L.h = take((size_t)count * n * 32);
+    L.ma = take((size_t)count * 64);
+    L.mb1 = take((size_t)count * 64);
+    L.mc = take((size_t)count * 64);
+    L.mh = take((size_t)count * 64);
+    L.mb2 = take((size_t)count * 128);
+    L.rs = take((size_t)count * 64);
+    uint64_t work = 2 * (uint64_t)count * n * 32, b = 0;
+    int rc;
+    for (const cw_g1_bases *g : {k->A.get(), k->B1.get(), k->C.get(), k->H.get()}) {
+        if (!g) continue;
+        if ((rc = cw_g1_msm_scratch_bytes(g, count, &b))) return rc;
+        work = std::max(work, b);
+    }
+    if ((rc = cw_g2_msm_scratch_bytes(k->B2.get(), count, &b))) return rc;
+    L.work = take(std::max(work, b));
+    L.total = at;
+    return CW_OK;
+}
+
+int cw_groth16_scratch_bytes(const cw_groth16_key *k, uint32_t count, uint64_t *bytes) {
+    if (!k || !bytes || count == 0) return fail(CW_EINVAL, "bad argument");
+    G16Layout L;
+    int rc = groth16_layout(k, count, L);
+    if (rc) return rc;
+    *bytes = L.total;
+    return CW_OK;
+}
+
+// (r, s) per proof: the caller's, checked to lie below r, or drawn from getrandom(2) by rejection below r
+static int groth16_blinding(const uint64_t *rs, u32 count, std::vector<uint64_t> &out) {
+    const U256 rr = make_field(CW_PRIME_BN128).q;
+    out.assign((size_t)count * 8, 0);
+    if (rs) {
+        for (size_t i = 0; i < (size_t)count * 2; ++i) {
+            U256 x;
+            memcpy(x.v, rs + 4 * i, 32);
+            if (!(x < rr))
+                return fail(CW_EINVAL, std::string(i & 1 ? "s" : "r") + " of proof " + std::to_string(i / 2) + " is not below r");
+        }
+        memcpy(out.data(), rs, out.size() * 8);
+        return CW_OK;
+    }
+    for (size_t i = 0; i < (size_t)count * 2; ++i) {
+        U256 x;
+        do {
+            uint8_t *p = (uint8_t *)x.v;
+            size_t got = 0;
+            while (got < 32) {
+                const ssize_t n = getrandom(p + got, 32 - got, 0);
+                if (n < 0) {
+                    if (errno == EINTR) continue;
+                    return fail(CW_EIO, std::string("getrandom: ") + strerror(errno));
+                }
+                got += (size_t)n;
+            }
+            x.v[3] &= (1ull << 62) - 1;   // r < 2^254: keep 254 bits, accept below r
+        } while (!(x < rr));
+        memcpy(out.data() + 4 * i, x.v, 32);
+    }
+    return CW_OK;
+}
+
+// steps 3-6 on `st`: the MSMs over h and over the witness rows, then the assembly kernel
+static int groth16_msms(cw_groth16_key *k, const uint64_t *rows, uint64_t stride, char *S, const G16Layout &L,
+                        const std::vector<uint64_t> &rs, u32 count, uint64_t *proofs, cudaStream_t st) {
+    auto at = [&](size_t off) { return (uint64_t *)(S + off); };
+    void *work = S + L.work;
+    CU(cudaMemcpyAsync(at(L.rs), rs.data(), rs.size() * 8, cudaMemcpyHostToDevice, st));   // (pageable: staged at once)
+    int rc;
+    if ((rc = cw_g1_msm_batch(k->H.get(), at(L.h), 1ull << k->log_n, count, at(L.mh), work, st))) return rc;
+    if ((rc = groth16_mark(k, 3, st))) return rc;
+    if ((rc = cw_g1_msm_batch(k->A.get(), rows, stride, count, at(L.ma), work, st))) return rc;
+    if ((rc = groth16_mark(k, 4, st))) return rc;
+    if ((rc = cw_g1_msm_batch(k->B1.get(), rows, stride, count, at(L.mb1), work, st))) return rc;
+    if ((rc = groth16_mark(k, 5, st))) return rc;
+    if ((rc = cw_g2_msm_batch(k->B2.get(), rows, stride, count, at(L.mb2), work, st))) return rc;
+    if ((rc = groth16_mark(k, 6, st))) return rc;
+    if (k->C) {
+        if ((rc = cw_g1_msm_batch(k->C.get(), rows + 4 * (k->n_public + 1), stride, count, at(L.mc), work, st))) return rc;
+    } else {
+        CU(cudaMemsetAsync(at(L.mc), 0, (size_t)count * 64, st));   // no private signals: the C term is infinity
+    }
+    if ((rc = groth16_mark(k, 7, st))) return rc;
+    groth16_launch_assemble(k->consts.get(), at(L.ma), at(L.mb1), at(L.mb2), at(L.mc), at(L.mh), at(L.rs), count, proofs, st);
+    CU(cudaGetLastError());
+    if ((rc = groth16_mark(k, 8, st))) return rc;
+    k->timed = true;
+    return CW_OK;
+}
+
+static int groth16_check_r1cs(const cw_groth16_key *k, cw_r1cs *r) {
+    if (r1cs_digest(r) != k->r1cs_digest) return fail(CW_EINVAL, "the R1CS is not the one the proving key was checked against");
+    return CW_OK;
+}
+
+int cw_groth16_prove_batch(cw_groth16_key *k, cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, const uint64_t *rs,
+                           uint64_t *proofs_dev, void *scratch_dev) {
+    if (!k || !r || !b || count == 0 || (uint64_t)first + count > b->batch) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(0, (const uint64_t *)scratch_dev, 0, count, proofs_dev, scratch_dev);
+    if (rc) return rc;
+    if (!b->ran) return fail(CW_ESTATE, "batch has not been run");
+    if ((rc = groth16_check_r1cs(k, r))) return rc;
+    if (b->c->tape.n_witness != k->n_vars) return fail(CW_EINVAL, "the batch's witness size differs from the key's nVars");
+    if (b->device != k->device) return fail(CW_EINVAL, "the batch and the proving key are on different devices");
+    std::vector<uint64_t> rsv;
+    if ((rc = groth16_blinding(rs, count, rsv))) return rc;
+    if ((rc = ensure_device(k->device))) return rc;
+    if ((rc = msm_check_pointers(k->device, (const uint64_t *)scratch_dev, proofs_dev, scratch_dev))) return rc;
+    G16Layout L;
+    if ((rc = groth16_layout(k, count, L))) return rc;
+    char *S = (char *)scratch_dev;
+    uint64_t *rows = (uint64_t *)(S + L.rows);
+    cudaStream_t st = b->stream.get();
+    k->timed = false;
+    if ((rc = groth16_mark(k, 0, st))) return rc;
+    if ((rc = cw_batch_expand_witness(b, first, count, rows))) return rc;
+    if ((rc = groth16_mark(k, 1, st))) return rc;
+    if ((rc = cw_r1cs_quotient_batch(r, b, first, count, (uint64_t *)(S + L.h), (uint64_t *)(S + L.work)))) return rc;
+    if ((rc = groth16_mark(k, 2, st))) return rc;
+    return groth16_msms(k, rows, k->n_vars, S, L, rsv, count, proofs_dev, b->stream.get());
+}
+
+int cw_groth16_prove_strided(cw_groth16_key *k, cw_r1cs *r, const uint64_t *witness_dev, uint64_t stride_elems, uint32_t count,
+                             const uint64_t *rs, uint64_t *proofs_dev, void *scratch_dev) {
+    if (!k || !r || stride_elems >> 32) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(k->n_vars, witness_dev, stride_elems, count, proofs_dev, scratch_dev);
+    if (rc) return rc;
+    if ((rc = groth16_check_r1cs(k, r))) return rc;
+    std::vector<uint64_t> rsv;
+    if ((rc = groth16_blinding(rs, count, rsv))) return rc;
+    if ((rc = ensure_device(k->device))) return rc;
+    if ((rc = msm_check_pointers(k->device, witness_dev, proofs_dev, scratch_dev))) return rc;
+    G16Layout L;
+    if ((rc = groth16_layout(k, count, L))) return rc;
+    char *S = (char *)scratch_dev;
+    DevPtr<unsigned long long> fb_d;
+    if ((rc = dev_alloc(fb_d, (size_t)count * 8))) return rc;
+    k->timed = false;
+    if ((rc = groth16_mark(k, 0, 0)) || (rc = groth16_mark(k, 1, 0))) return rc;   // (no expansion: the rows are given)
+    if ((rc = quotient_on_store(r, k->device, nullptr, dense_store(witness_dev, stride_elems, count), 0, count,
+                                (uint64_t *)(S + L.h), (uint64_t *)(S + L.work), fb_d.get(), 0)))
+        return rc;
+    if ((rc = groth16_mark(k, 2, 0))) return rc;
+    if ((rc = groth16_msms(k, witness_dev, stride_elems, S, L, rsv, count, proofs_dev, 0))) return rc;
+    CU(cudaStreamSynchronize(0));
+    return CW_OK;
+}
+
+int cw_groth16_last_ms(cw_groth16_key *k, float ms[8]) {
+    if (!k || !ms) return fail(CW_EINVAL, "null argument");
+    if (!k->timed) return fail(CW_ESTATE, "no prove call has been issued on this key");
+    CU(cudaSetDevice(k->device));
+    CU(cudaEventSynchronize(k->ev[G16_STAGES].get()));
+    for (int i = 0; i < G16_STAGES; ++i) CU(cudaEventElapsedTime(&ms[i], k->ev[i].get(), k->ev[i + 1].get()));
+    return CW_OK;
+}
+
+int cw_groth16_proof_json(const uint64_t proof[32], char *out, size_t cap, size_t *len) {
+    if (!proof) return fail(CW_EINVAL, "null argument");
+    return copy_text(groth16_proof_json(proof), out, cap, len);
+}
+
+int cw_groth16_public_json(const uint64_t *public_signals, uint32_t n_public, char *out, size_t cap, size_t *len) {
+    if (!public_signals && n_public) return fail(CW_EINVAL, "null argument");
+    return copy_text(groth16_public_json(public_signals, n_public), out, cap, len);
 }
 
 // readWitness side of the file boundary: the 32-byte entries of a .wtns (written by this library, the reference

@@ -446,6 +446,30 @@ static std::string u256_decimal(const uint64_t *v) {
     return out;
 }
 
+static bool all_zero(const uint64_t *v, int n) {
+    for (int i = 0; i < n; ++i)
+        if (v[i]) return false;
+    return true;
+}
+
+// snarkjs writes affine points in projective form [x, y, "1"]; the point at infinity is ["0", "1", "0"] in G1 and
+// [["0", "0"], ["1", "0"], ["0", "0"]] in G2
+std::string groth16_proof_json(const uint64_t *p) {
+    auto d = [&](int k) { return "\"" + u256_decimal(p + 4 * k) + "\""; };
+    auto g1 = [&](int k) {
+        return all_zero(p + 4 * k, 8) ? std::string("[\"0\",\"1\",\"0\"]") : "[" + d(k) + "," + d(k + 1) + ",\"1\"]";
+    };
+    const std::string b = all_zero(p + 8, 16) ? std::string("[[\"0\",\"0\"],[\"1\",\"0\"],[\"0\",\"0\"]]")
+                                              : "[[" + d(2) + "," + d(3) + "],[" + d(4) + "," + d(5) + "],[\"1\",\"0\"]]";
+    return "{\"pi_a\":" + g1(0) + ",\"pi_b\":" + b + ",\"pi_c\":" + g1(6) + ",\"protocol\":\"groth16\",\"curve\":\"bn128\"}";
+}
+
+std::string groth16_public_json(const uint64_t *signals, uint32_t n) {
+    std::string out = "[";
+    for (uint32_t i = 0; i < n; ++i) out += (i ? ",\"" : "\"") + u256_decimal(signals + 4 * (size_t)i) + "\"";
+    return out + "]";
+}
+
 // LogBucket (log_bucket.rs:104-162): the arguments of a call separated by one blank, values as decimals, a newline after the last
 std::string format_log(const Tape &t, const uint64_t *witness) {
     std::string out;

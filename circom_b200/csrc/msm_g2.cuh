@@ -220,7 +220,7 @@ struct MsmG2XyzzItems {
 
 }  // namespace cw
 
-#if defined(__CUDACC__)
+#if defined(__CUDACC__) && !defined(CW_MSM_NO_G2_KERNELS)   // (groth16.cu uses the point functions only)
 // ---- kernels (sm_90a) -------------------------------------------------------------------------------------------------
 // The digits and the sort are msm.cuh's (they do not depend on the group).  The bucket type is four times the G1 one, so
 // the kernels run MSM_G2_THREADS threads per CTA, which lets ptxas use up to 255 registers per thread (DESIGN section 4).

@@ -167,5 +167,9 @@ void read_wtns(const std::string &path, int &prime_id, std::vector<uint64_t> &wi
 void write_sym(const Tape &t, const std::string &path);
 // the text the log() calls of the circuit print for one witness (n_witness x 4 u64), as the reference calculator prints it
 std::string format_log(const Tape &t, const uint64_t *witness);
+// snarkjs' proof.json of one proof ([32] u64: A x, y | B x.c0, x.c1, y.c0, y.c1 | C x, y, canonical; zeros = infinity) and
+// public.json of n public signals ([n][4] u64 canonical), as compact JSON with decimal strings
+std::string groth16_proof_json(const uint64_t *proof);
+std::string groth16_public_json(const uint64_t *signals, uint32_t n);
 
 }  // namespace cw

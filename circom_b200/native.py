@@ -99,6 +99,16 @@ def _load() -> ctypes.CDLL:
         "cw_g2_bases_destroy": (None, [P]),
         "cw_g2_msm_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
         "cw_g2_msm_batch": (c_int, [P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_groth16_key_create": (c_int, [c_void_p, c_size_t, P, c_int, POINTER(P)]),
+        "cw_groth16_key_destroy": (None, [P]),
+        "cw_groth16_key_info": (c_int, [P, POINTER(c_uint64)]),
+        "cw_groth16_key_ic": (c_int, [P, c_void_p]),
+        "cw_groth16_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
+        "cw_groth16_prove_batch": (c_int, [P, P, P, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_groth16_prove_strided": (c_int, [P, P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_groth16_last_ms": (c_int, [P, POINTER(c_float)]),
+        "cw_groth16_proof_json": (c_int, [c_void_p, c_char_p, c_size_t, POINTER(c_size_t)]),
+        "cw_groth16_public_json": (c_int, [c_void_p, c_uint32, c_char_p, c_size_t, POINTER(c_size_t)]),
         "cw_comm_unique_id": (c_int, [c_void_p]),
         "cw_comm_init": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),
         "cw_comm_from_nccl": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(P)]),

@@ -620,6 +620,154 @@ class G2Bases:
                 for i in range(count)]
 
 
+def _proof_from_limbs(v: Sequence[int]):
+    """one proof's 8 canonical coordinates -> (A, B, C): A, C = (x, y), B = ((x0, x1), (y0, y1)); None = infinity"""
+    A = None if not any(v[0:2]) else (v[0], v[1])
+    B = None if not any(v[2:6]) else ((v[2], v[3]), (v[4], v[5]))
+    C = None if not any(v[6:8]) else (v[6], v[7])
+    return A, B, C
+
+
+def _rs_array(rs, count: int):
+    """(r, s) per proof as a [count][2][4] uint64 array, or None (the library draws them)"""
+    if rs is None:
+        return None
+    if isinstance(rs, np.ndarray):
+        return np.ascontiguousarray(rs, dtype=np.uint64).reshape(count, 2, 4)
+    assert len(rs) == count, "one (r, s) pair per proof"
+    return ints_to_limbs([x for pair in rs for x in pair]).reshape(count, 2, 4)
+
+
+class Groth16Key:
+    """A BN254 Groth16 proving key on the device (cw_groth16_key_*, include/circom_b200.h), read from the bytes of a
+    snarkjs .zkey - or from its path - and checked against the R1CS `r1cs` (an R1cs).  Proofs are [32] uint64 rows:
+    A (x, y) | B (x.c0, x.c1, y.c0, y.c1) | C (x, y), canonical, zeros = infinity.  rs: (r, s) per proof - ints, or
+    uint64 [count][2][4] - or None for blinding drawn by the library (what zero knowledge needs)."""
+
+    def __init__(self, zkey: Union[bytes, str, os.PathLike], r1cs: "R1cs", device: int = 0):
+        if not isinstance(zkey, (bytes, bytearray, memoryview)):
+            with open(zkey, "rb") as f:
+                zkey = f.read()
+        data = bytes(zkey)
+        self.device = device
+        self.r1cs = r1cs
+        self._h = ctypes.c_void_p()
+        check(lib.cw_groth16_key_create(data, len(data), r1cs._h, device, ctypes.byref(self._h)))
+        info = (ctypes.c_uint64 * 4)()
+        check(lib.cw_groth16_key_info(self._h, info))
+        self.info = {"n_vars": info[0], "n_public": info[1], "log2_domain": info[2], "n_coefs": info[3]}
+        self.n_vars, self.n_public = info[0], info[1]
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            lib.cw_groth16_key_destroy(h)
+
+    def ic(self) -> List[Optional[tuple]]:
+        """the verifier's IC points (nPublic + 1 of them), affine (x, y) or None"""
+        out = np.zeros((self.n_public + 1, 2, 4), dtype=np.uint64)
+        check(lib.cw_groth16_key_ic(self._h, out.ctypes.data))
+        v = limbs_to_ints(out)
+        return [None if (x, y) == (0, 0) else (x, y) for x, y in zip(v[0::2], v[1::2])]
+
+    def scratch_bytes(self, count: int) -> int:
+        b = ctypes.c_uint64()
+        check(lib.cw_groth16_scratch_bytes(self._h, count, ctypes.byref(b)))
+        return b.value
+
+    def prove_batch(self, batch: "Batch", first: int, count: int, proofs_ptr: int, scratch_ptr: int, rs=None) -> None:
+        """proofs of instances [first, first + count) of a batch that has run into device [count][32] uint64;
+        asynchronous on the batch stream.  Instances whose witness violates the R1CS give proofs that do not verify."""
+        a = _rs_array(rs, count)
+        check(lib.cw_groth16_prove_batch(self._h, self.r1cs._h, batch._h, first, count, None if a is None else a.ctypes.data,
+                                         ctypes.c_void_p(proofs_ptr), ctypes.c_void_p(scratch_ptr)))
+
+    def last_ms(self) -> dict:
+        """device ms of the stages of the last prove call (waits for it): expansion, quotient, H, A, B1, B2, C, assembly"""
+        ms = (ctypes.c_float * 8)()
+        check(lib.cw_groth16_last_ms(self._h, ms))
+        return dict(zip(("expansion", "quotient", "H", "A", "B1", "B2", "C", "assembly"), (float(x) for x in ms)))
+
+    def prove(self, witness_ptr: int, stride: Optional[int], count: int, proofs_ptr: int, scratch_ptr: int, rs=None) -> None:
+        """proofs of `count` dense witness rows on the device, `stride` 32-byte elements apart (None: nVars); returns
+        when the proofs are written"""
+        a = _rs_array(rs, count)
+        check(lib.cw_groth16_prove_strided(self._h, self.r1cs._h, ctypes.c_void_p(witness_ptr), stride or self.n_vars, count,
+                                           None if a is None else a.ctypes.data, ctypes.c_void_p(proofs_ptr),
+                                           ctypes.c_void_p(scratch_ptr)))
+
+    def _chunk(self, count: int, max_scratch: Optional[int]) -> int:
+        import torch
+        budget = max_scratch if max_scratch is not None else torch.cuda.mem_get_info(self.device)[0] // 2
+        c = count
+        while c > 1 and self.scratch_bytes(c) > budget:
+            c = (c + 1) // 2
+        return c
+
+    def prove_host(self, source, rs=None, first: int = 0, count: Optional[int] = None,
+                   max_scratch: Optional[int] = None) -> list:
+        """proofs as Python ints, [(A, B, C)] (see _proof_from_limbs), in chunks whose scratch fits max_scratch bytes
+        (None: half the free device memory).  source: a Batch that has run - instances [first, first + count), refused
+        if any of them has a non-zero status - or host witness rows (uint64 [count][nVars][4], or lists of ints)."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if isinstance(source, Batch):
+            count = source.batch - first if count is None else count
+            st = source.status()[first:first + count]
+            if (st != 0).any():
+                bad = int(np.nonzero(st)[0][0])
+                raise CwError(native.CW_ESTATE, "instance %d has status %d: its witness is not valid" % (first + bad, st[bad]))
+            rows = None
+        else:
+            rows = source if isinstance(source, np.ndarray) else ints_to_limbs([x for row in source for x in row])
+            rows = np.ascontiguousarray(rows, dtype=np.uint64).reshape(-1, self.n_vars, 4)
+            count = rows.shape[0]
+        a = _rs_array(rs, count)
+        chunk = self._chunk(count, max_scratch)
+        out = []
+        scratch = torch.empty(self.scratch_bytes(chunk), dtype=torch.uint8, device=dev)
+        for i0 in range(0, count, chunk):
+            cn = min(chunk, count - i0)
+            proofs = torch.empty((cn, 32), dtype=torch.int64, device=dev)
+            part = None if a is None else a[i0:i0 + cn]
+            # (torch's allocations are ordered on its current stream; the batch stream is another one)
+            torch.cuda.current_stream(dev).synchronize()
+            if rows is None:
+                self.prove_batch(source, first + i0, cn, proofs.data_ptr(), scratch.data_ptr(), part)
+                source.sync()
+            else:
+                w = torch.from_numpy(rows[i0:i0 + cn].view(np.int64)).to(dev)
+                self.prove(w.data_ptr(), self.n_vars, cn, proofs.data_ptr(), scratch.data_ptr(), part)
+            v = limbs_to_ints(proofs.cpu().numpy().view(np.uint64))
+            out += [_proof_from_limbs(v[8 * i:8 * i + 8]) for i in range(cn)]
+        return out
+
+    @staticmethod
+    def proof_json(proof) -> str:
+        """snarkjs' proof.json text of one proof: a (A, B, C) tuple as prove_host returns, or its [32] uint64 row"""
+        if isinstance(proof, np.ndarray):
+            row = np.ascontiguousarray(proof, dtype=np.uint64).reshape(32)
+        else:
+            A, B, C = proof
+            row = ints_to_limbs(list(A or (0, 0)) + ([0] * 4 if B is None else [B[0][0], B[0][1], B[1][0], B[1][1]])
+                                + list(C or (0, 0))).reshape(32)
+        return _text(lambda buf, cap, ln: lib.cw_groth16_proof_json(row.ctypes.data, buf, cap, ln))
+
+    @staticmethod
+    def public_json(signals: Sequence[int]) -> str:
+        """snarkjs' public.json text of the public signals w_1..w_nPublic"""
+        arr = ints_to_limbs(list(signals)) if len(signals) else np.zeros((1, 4), dtype=np.uint64)
+        return _text(lambda buf, cap, ln: lib.cw_groth16_public_json(arr.ctypes.data, len(signals), buf, cap, ln))
+
+
+def _text(call) -> str:
+    n = ctypes.c_size_t()
+    check(call(None, 0, ctypes.byref(n)))
+    buf = ctypes.create_string_buffer(n.value + 1)
+    check(call(buf, n.value + 1, ctypes.byref(n)))
+    return buf.value.decode()
+
+
 class WitnessCalculator:
     """`builder(code, options)` of witness_calculator.js:1-106, for a circuit description."""
 

@@ -358,6 +358,63 @@ int cw_g2_msm_scratch_bytes(const cw_g2_bases *b, uint32_t count, uint64_t *byte
 int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
                     uint64_t *out_dev, void *scratch_dev, void *stream);
 
+/* ---- Groth16 proofs on BN254 -----------------------------------------------------------------------------------------
+ * Whole proofs for a batch of witnesses: the quotient above, the five MSMs above and an assembly kernel.  Per proof, with
+ * MA, MB1, MC the G1 MSMs over the witness (C over its private part, w_{nPublic+1..}), MB2 the G2 MSM and MH the G1 MSM
+ * of h over the key's H points:
+ *   A = alpha1 + MA + r delta1,  B = beta2 + MB2 + s delta2,  C = MC + MH + s A + r (beta1 + MB1)
+ * which is snarkjs' and rapidsnark's C = MC + MH + s A + r B1 - r s delta1.
+ *
+ * The proving key is read from the bytes of a snarkjs Groth16 .zkey (all little-endian): "zkey", u32 version = 1,
+ * u32 nSections, then (u32 id, u64 size, payload) records in any order.  Section 1: u32 protocol = 1.  Section 2: u32 n8q,
+ * q, u32 n8r, r, u32 nVars, u32 nPublic, u32 domainSize, alpha1, beta1, beta2, gamma2, delta1, delta2.  Section 3: IC,
+ * nPublic + 1 G1 points.  Section 4: u32 nCoefs, then (u32 matrix, u32 constraint, u32 signal, 32-byte value) records.
+ * Sections 5-9: A (nVars G1), B1 (nVars G1), B2 (nVars G2), C (nVars - nPublic - 1 G1), H (domainSize G1).  Section 10
+ * (contributions) is ignored.  Coordinates are Montgomery images mod q with R = 2^256; G1 points are (x, y), 64 bytes,
+ * G2 points (x.c0, x.c1, y.c0, y.c1), 128 bytes; all zeros is infinity.  This layout is written from snarkjs' format
+ * description: byte compatibility with a file snarkjs wrote is not verified by this library.
+ *
+ * H is taken in the convention of the quotient above: H_j multiplies h_j, the j-th evaluation on the odd coset.
+ * Zero knowledge rests on the blinding (r, s): pass rs = NULL to draw them from getrandom(2).  A witness that does not
+ * satisfy the R1CS gives a proof that does not verify (as in snarkjs and rapidsnark): check the batch status first. */
+typedef struct cw_groth16_key cw_groth16_key;
+/* Parse and check the key on the host before any device is touched; every refusal is CW_EINVAL and cw_last_error names
+ * it: magic, version, protocol; n8q = n8r = 32 with q, r BN254's fields; every section 1-9 present once, with exactly
+ * the size the header implies (64-bit arithmetic); nPublic < nVars; every coordinate below q and every point on its
+ * curve; nVars = the R1CS's wires, nPublic and domainSize as cw_r1cs_qap_info gives them, and the (matrix, constraint,
+ * signal) triples of section 4, as a multiset, the nonzero A and B terms of r plus the rows A[m + j][j], j <= nPublic
+ * (a key of another circuit of the same size is refused; the coefficient values are not compared: their encoding in
+ * section 4 could not be confirmed against a snarkjs file).  Then the base sets go to `device` (CW_ENODEV without one).
+ * The key remembers a digest of r's constraints: the prove calls refuse another R1CS. */
+int cw_groth16_key_create(const void *zkey, size_t len, const cw_r1cs *r, int device, cw_groth16_key **out);
+void cw_groth16_key_destroy(cw_groth16_key *k);
+/* info = {nVars, nPublic, log2 domainSize, nCoefs} */
+int cw_groth16_key_info(const cw_groth16_key *k, uint64_t info[4]);
+/* the verifier's IC points: out[nPublic + 1][2][4] u64 canonical affine, (0, 0) = infinity */
+int cw_groth16_key_ic(const cw_groth16_key *k, uint64_t *out);
+/* device scratch of the prove calls for `count` proofs: witness rows + h + MSM results + max(quotient, MSM) work */
+int cw_groth16_scratch_bytes(const cw_groth16_key *k, uint32_t count, uint64_t *bytes);
+/* proofs_dev: [count][32] u64 = A (x, y) | B (x.c0, x.c1, y.c0, y.c1) | C (x, y), canonical affine, zeros = infinity.
+ * rs: host [count][2][4] u64 canonical (r_c, s_c), each < r, or NULL: drawn with getrandom(2), rejection-sampled below r.
+ * Device pointers 32-byte aligned, on the key's device.  r must be the R1CS the key was checked against (CW_EINVAL).
+ * _batch proves instances [first, first + count) of a batch that has run, asynchronously on the batch stream (no host
+ * synchronisation: expansion of the rows, quotient, the MSMs, assembly).  _strided proves dense witness rows on the
+ * device (row i at witness_dev + i * stride_elems * 4, stride_elems >= nVars; e.g. .wtns files read with cw_wtns_read),
+ * on the legacy default stream, and returns when the proofs are written. */
+int cw_groth16_prove_batch(cw_groth16_key *k, cw_r1cs *r, cw_batch *b, uint32_t first, uint32_t count, const uint64_t *rs,
+                           uint64_t *proofs_dev, void *scratch_dev);
+int cw_groth16_prove_strided(cw_groth16_key *k, cw_r1cs *r, const uint64_t *witness_dev, uint64_t stride_elems,
+                             uint32_t count, const uint64_t *rs, uint64_t *proofs_dev, void *scratch_dev);
+/* device time in ms of the stages of the last prove call on k: expansion (0 for _strided), quotient, the H, A, B1, B2 and
+ * C MSMs, assembly (events recorded on the call's stream; waits for the call to finish).  CW_ESTATE before any call. */
+int cw_groth16_last_ms(cw_groth16_key *k, float ms[8]);
+/* snarkjs' proof.json of one proof (host [32] u64 as above): {"pi_a": [x, y, "1"], "pi_b": [[x.c0, x.c1], [y.c0, y.c1],
+ * ["1", "0"]], "pi_c": [x, y, "1"], "protocol": "groth16", "curve": "bn128"} with decimal strings, compact; infinity as
+ * ["0", "1", "0"] (G1) or [["0", "0"], ["1", "0"], ["0", "0"]] (G2).  public.json of the public signals w_1..w_nPublic
+ * (host [n_public][4] u64 canonical): ["w_1", ...].  Writes at most cap bytes incl. the terminator; *len = whole length. */
+int cw_groth16_proof_json(const uint64_t proof[32], char *out, size_t cap, size_t *len);
+int cw_groth16_public_json(const uint64_t *public_signals, uint32_t n_public, char *out, size_t cap, size_t *len);
+
 /* ---- multi-GPU: one process per GPU, independent inputs sharded over the ranks ---------------------------
  * The reference has no distributed mode (Circom_CalcWit is per-process state, calcwit.cpp:26-45).  Here rank 0
  * lowers the circuit and broadcasts the lowered form once; every rank runs its shard; witnesses are gathered in
