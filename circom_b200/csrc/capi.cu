@@ -31,6 +31,7 @@
 #include "kernels.cuh"
 #include "msm.cuh"
 #include "msm_g2.h"
+#include "msm_bls12381.h"
 #include "groth16.h"
 #include "tape_calls.h"
 #include "tape.h"
@@ -117,6 +118,7 @@ int ensure_device(int device) {
         CU(cudaMemcpyToSymbol(c_fr, h, sizeof(h)));
         CU(tape_calls_set_params(h, sizeof(h)));
         CU(msm_g2_set_params(h, sizeof(h)));
+        CU(msm_bls12381_set_params());
         CU(groth16_set_params(h, sizeof(h)));
         g_dev_ready[device] = true;
     }
@@ -2090,6 +2092,86 @@ int cw_g2_msm_batch(cw_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride
             lv ^= 1;
         }
         msm_g2_launch_reduce(buckets, p.B, n_win, S + p.segs, S + p.wins, p.W, p.c, cn, (uint4 *)(out_dev + 16 * (size_t)i0), st);
+        CU(cudaGetLastError());
+    }
+    return CW_OK;
+}
+
+// ---- multi-scalar multiplication on G1 of BLS12-381 (msm_bls12381.cuh, kernels in msm_bls12381.cu) -------------------
+struct cw_bls12381_g1_bases {
+    int device = 0;
+    uint64_t n = 0;
+    DevPtr<u32> pts;   // [n][24] u32: Montgomery x, y (12 limbs each); (0, 0) = infinity
+};
+
+int cw_bls12381_g1_bases_create(const uint64_t *points, uint64_t n, int device, cw_bls12381_g1_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    std::vector<u32> mont(24 * n);
+    for (uint64_t i = 0; i < n; ++i) {
+        const int bad = bls12381_g1_point_mont(points + 12 * i, &mont[24 * i]);
+        if (bad == 1) return fail(CW_EINVAL, "point " + std::to_string(i) + ": a coordinate is not below q");
+        if (bad) return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the curve y^2 = x^3 + 4");
+    }
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    auto b = std::make_unique<cw_bls12381_g1_bases>();
+    b->device = device;
+    b->n = n;
+    if ((rc = upload(b->pts, mont.data(), mont.size() * 4))) return rc;
+    *out = b.release();
+    return CW_OK;
+}
+
+void cw_bls12381_g1_bases_destroy(cw_bls12381_g1_bases *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    delete b;
+}
+
+int cw_bls12381_g1_msm_scratch_bytes(const cw_bls12381_g1_bases *b, uint32_t count, uint64_t *bytes) {
+    if (!b || !bytes || count == 0) return fail(CW_EINVAL, "bad argument");
+    int rc = ensure_device(b->device);
+    if (rc) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_BLS_POINT_BYTES))) return rc;
+    *bytes = p.total;
+    return CW_OK;
+}
+
+int cw_bls12381_g1_msm_batch(cw_bls12381_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                             uint64_t *out_dev, void *scratch_dev, void *stream) {
+    if (!b) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(b->n, scalars_dev, stride_elems, count, out_dev, scratch_dev);
+    if (rc) return rc;
+    if ((rc = ensure_device(b->device))) return rc;
+    if ((rc = msm_check_pointers(b->device, scalars_dev, out_dev, scratch_dev))) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_BLS_POINT_BYTES))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char *S = (char *)scratch_dev;
+    const u32 n = (u32)b->n;
+    for (u32 i0 = 0; i0 < count; i0 += p.chunk) {
+        const u32 cn = std::min(p.chunk, count - i0), n_win = cn * p.W;
+        const uint64_t N = (uint64_t)n_win * n;
+        if ((rc = msm_sorted_digits(p, S, scalars_dev, stride_elems, n, i0, cn, st))) return rc;
+        void *buckets = S + p.buckets;
+        CU(cudaMemsetAsync(buckets, 0, (size_t)n_win * p.B * MSM_BLS_POINT_BYTES, st));
+        // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
+        uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
+        int lv = 0;
+        msm_bls12381_launch_runs(true, (const u32 *)(S + p.keys[1]), (const u32 *)(S + p.vals[1]), b->pts.get(), nullptr, N,
+                                 p.c, buckets, (u32 *)(S + p.lv_keys[0]), S + p.lv_pts[0], st);
+        while (threads > 1) {
+            items = msm_level_out(items);
+            threads = (items + MSM_RUN - 1) / MSM_RUN;
+            msm_bls12381_launch_runs(false, (const u32 *)(S + p.lv_keys[lv]), nullptr, nullptr, S + p.lv_pts[lv], items, p.c,
+                                     buckets, (u32 *)(S + p.lv_keys[lv ^ 1]), S + p.lv_pts[lv ^ 1], st);
+            lv ^= 1;
+        }
+        msm_bls12381_launch_reduce(buckets, p.B, n_win, S + p.segs, S + p.wins, p.W, p.c, cn,
+                                   (uint4 *)(out_dev + 12 * (size_t)i0), st);
         CU(cudaGetLastError());
     }
     return CW_OK;

@@ -136,10 +136,11 @@ CW_HD void xyzz_add(Xyzz &a, const Xyzz &b, const FrParams &P) {
     fr_sub(a.y, q, t, P);               // Y3 = R (Q - X3) - S1 PPP
 }
 
-// r = k p for a small k (double-and-add from the top bit); Pt: Xyzz here, XyzzG2 in msm_g2.cuh (the point functions are
-// found by overloading)
-template <class Pt>
-CW_HD void xyzz_mul_small(Pt &r, const Pt &p, u32 k, const FrParams &P) {
+// r = k p for a small k (double-and-add from the top bit); Pt: Xyzz here, XyzzG2 in msm_g2.cuh, Xyzz381 in
+// msm_bls12381.cuh (the point functions are found by overloading); Par: the field's parameter record (FrParams, or
+// Fp381Params for the 381-bit field)
+template <class Pt, class Par>
+CW_HD void xyzz_mul_small(Pt &r, const Pt &p, u32 k, const Par &P) {
     xyzz_inf(r);
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
@@ -235,7 +236,8 @@ struct MsmXyzzItems {
 
 // one run's sum at the end of a thread's range walk: a whole bucket goes to `buckets`, a run that continues past the
 // range goes to the thread's slot (first run: slot 0, last run: slot 1).  The run machinery below does not depend on the
-// group: Pt is the bucket type (Xyzz for G1, XyzzG2 for G2 in msm_g2.cuh).
+// group: Pt is the bucket type (Xyzz for G1, XyzzG2 for G2 in msm_g2.cuh, Xyzz381 for BLS12-381 G1 in msm_bls12381.cuh)
+// and Par the parameter record its field functions take.
 template <class Pt>
 struct MsmRunOutT {
     Pt *buckets;
@@ -266,8 +268,8 @@ CW_HD void msm_emit(const MsmRunOutT<Pt> &o, uint64_t t, u32 c, u32 key, const P
 }
 
 // thread t of a level over N sorted items: sums the runs of [t MSM_RUN, (t + 1) MSM_RUN)
-template <class Items, class Pt>
-CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const MsmRunOutT<Pt> &o, const FrParams &P) {
+template <class Items, class Pt, class Par>
+CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const MsmRunOutT<Pt> &o, const Par &P) {
     const uint64_t lo = t * MSM_RUN, hi = lo + MSM_RUN < N ? lo + MSM_RUN : N;
     const u32 before = lo > 0 ? it.keys[lo - 1] : MSM_NONE, after = hi < N ? it.keys[hi] : MSM_NONE;
     u32 slot_key[2] = {MSM_NONE, MSM_NONE};
@@ -297,8 +299,8 @@ CW_HD void msm_sum_runs(const Items &it, uint64_t N, uint64_t t, u32 c, const Ms
 CW_HD uint64_t msm_level_out(uint64_t N) { return 2 * ((N + MSM_RUN - 1) / MSM_RUN); }
 
 // buckets [lo, lo + m) of one window (bucket b holds digit b + 1): sum_{b} (b + 1) B_b over the segment
-template <class Pt>
-CW_HD void msm_bucket_segment(Pt &out, const Pt *win, u32 lo, u32 m, const FrParams &P) {
+template <class Pt, class Par>
+CW_HD void msm_bucket_segment(Pt &out, const Pt *win, u32 lo, u32 m, const Par &P) {
     Pt run, tot, b;
     xyzz_inf(run);
     xyzz_inf(tot);
@@ -315,8 +317,8 @@ CW_HD void msm_bucket_segment(Pt &out, const Pt *win, u32 lo, u32 m, const FrPar
 }
 
 // sum_w 2^(c w) S_w (Horner's rule from the top window)
-template <class Pt>
-CW_HD void msm_horner(Pt &acc, const Pt *win, u32 W, u32 c, const FrParams &P) {
+template <class Pt, class Par>
+CW_HD void msm_horner(Pt &acc, const Pt *win, u32 W, u32 c, const Par &P) {
     msm_ld_xyzz(acc, win + (W - 1));
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1

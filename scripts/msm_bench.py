@@ -74,11 +74,15 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--sweep", default="20:14-19,21:15-19", help="log2 n:c range pairs timed at count 8, uniform scalars")
     ap.add_argument("--pipeline", type=int, default=64, help="headline witnesses for quotient + H MSM (0: skip)")
-    ap.add_argument("--group", choices=("g1", "g2"), default="g1",
-                    help="g2: time cw_g2_msm_batch, and the pipeline leg is B1 + B2 over expanded headline witness rows")
+    ap.add_argument("--group", choices=("g1", "g2", "bls12381"), default="g1",
+                    help="g2: time cw_g2_msm_batch, and the pipeline leg is B1 + B2 over expanded headline witness rows; "
+                         "bls12381: time cw_bls12381_g1_msm_batch beside cw_g1_msm_batch of the same shape, and the "
+                         "pipeline leg is quotient + H MSM of BLS12-381 Sha256(512) (config C4)")
     args = ap.parse_args()
     if args.group == "g2":
         return main_g2(args)
+    if args.group == "bls12381":
+        return main_bls(args)
     import torch
     from circom_b200 import native
     from circom_b200.circuit import CircuitDesc
@@ -335,6 +339,142 @@ def main_g2(args):
                           "expand_ms_per_witness": round(e_ms / cnt, 3), "b1_g1_msm_ms_per_witness": round(b1_ms / cnt, 3),
                           "b2_g2_msm_ms_per_witness": round(b2_ms / cnt, 3),
                           "b2_over_b1": round(b2_ms / b1_ms, 2)}), flush=True)
+    print(json.dumps({"card_after": card()}), flush=True)
+
+
+def main_bls(args):
+    """BLS12-381 G1 against BN254 G1 at the same shapes, in the same call.  The product counts are 381-bit products
+    (12-limb CIOS); a 12-limb product is about (12/8)^2 = 2.25 times the integer work of an 8-limb one, so that ratio is
+    printed next to the measured time ratio as an expectation, not as a bound."""
+    import torch
+    from circom_b200.circuit import CircuitDesc
+    from circom_b200 import circuits as C
+    from circom_b200.witness_calculator import Circuit, Batch, Bls12381G1Bases, G1Bases, R1cs, limbs_to_ints
+    from oracle import g1_model as GM
+    from tests import bls12381_model as BM
+
+    print(json.dumps({"card": card(), "group": "bls12381"}), flush=True)
+    logs = [int(x) for x in args.logs.split(",")]
+    counts = [int(x) for x in args.counts.split(",")]
+    n_max = 1 << max(logs + [21])
+    rng = random.Random(1)
+    bpts, _ = BM.multiples(rng.randrange(BM.R), rng.randrange(BM.R), n_max)
+    bls_np = np.frombuffer(b"".join(x.to_bytes(48, "little") + y.to_bytes(48, "little") for x, y in bpts),
+                           dtype=np.uint64).reshape(-1, 2, 6)
+    del bpts
+    gpts, _ = GM.multiples(rng.randrange(GM.R), rng.randrange(GM.R), n_max)
+    bn_np = np.frombuffer(b"".join(x.to_bytes(32, "little") + y.to_bytes(32, "little") for x, y in gpts),
+                          dtype=np.uint64).reshape(-1, 2, 4)
+    del gpts
+
+    # bit-heavy rows: expanded BLS12-381 Sha256compression witnesses
+    d = CircuitDesc("bls12381")
+    d.set_main(C.sha256_compression(d))
+    sc = Circuit(d, fuse=True)
+    sb = Batch(sc, max(counts))
+    ins = np.zeros((max(counts), sc.n_inputs, 4), dtype=np.uint64)
+    ins[:, :, 0] = np.random.default_rng(0).integers(0, 2, size=(max(counts), sc.n_inputs), dtype=np.uint64)
+    sb.set_inputs(ins)
+    sb.run()
+    wrows = sb.witness()
+    del sb
+
+    def time_msm(b, s, n, cnt, width):
+        out = torch.zeros((cnt, 2, width), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(b.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.reps):
+            b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / args.reps
+
+    for k in logs:
+        n = 1 << k
+        bb, gb = Bls12381G1Bases(bls_np[:n]), G1Bases(bn_np[:n])
+        c = window_bits(n)
+        for kind in ("uniform", "bits"):
+            for cnt in counts:
+                if kind == "uniform":
+                    s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+                    live = cnt * n * windows(c)
+                else:
+                    reps = -(-n // wrows.shape[1])
+                    host = np.concatenate([np.tile(wrows[i % wrows.shape[0]], (reps, 1))[:n][None] for i in range(cnt)])
+                    s = torch.from_numpy(host.view(np.int64)).cuda()
+                    live = 0
+                    for i in range(cnt):
+                        row = limbs_to_ints(wrows[i % wrows.shape[0]])
+                        per = sum(nonzero_digits(v, c) for v in row)
+                        full, part = divmod(n, len(row))
+                        live += full * per + sum(nonzero_digits(v, c) for v in row[:part])
+                ms_bls = time_msm(bb, s, n, cnt, 6)
+                ms_bn = time_msm(gb, s, n, cnt, 4)
+                print(json.dumps({"what": "bls12381_g1_msm", "scalars": kind, "log2_n": k, "c": c, "count": cnt,
+                                  "ms_call": round(ms_bls, 3), "ms_per_msm": round(ms_bls / cnt, 3),
+                                  "p381_products_per_msm": products(n, c, live // cnt),
+                                  "bn254_g1_ms_per_msm": round(ms_bn / cnt, 3), "bls_over_bn": round(ms_bls / ms_bn, 2),
+                                  "limb_work_ratio_expected": 2.25}), flush=True)
+                del s
+                torch.cuda.empty_cache()
+        del bb, gb
+
+    for part in filter(None, args.sweep.split(",")):
+        k, rng_c = part.split(":")
+        lo, hi = (int(x) for x in rng_c.split("-"))
+        n, cnt = 1 << int(k), 8
+        b = Bls12381G1Bases(bls_np[:n])
+        s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+        for c in range(lo, hi + 1):
+            os.environ["CW_MSM_WINDOW"] = str(c)
+            ms = time_msm(b, s, n, cnt, 6)
+            print(json.dumps({"what": "window_sweep_bls12381", "log2_n": int(k), "c": c, "rule_c": window_bits(n),
+                              "count": cnt, "ms_per_msm": round(ms / cnt, 3)}), flush=True)
+        os.environ.pop("CW_MSM_WINDOW", None)
+        del b, s
+        torch.cuda.empty_cache()
+
+    # the pipeline leg of config C4 (Sha256 of 512 bits over BLS12-381): quotient, then the H MSM on the batch stream
+    if args.pipeline:
+        cnt = args.pipeline
+        d = CircuitDesc("bls12381")
+        d.set_main(C.sha256(d, 512))
+        r_ = np.random.default_rng(0)
+        ins = np.zeros((cnt, d.main.n_in, 4), dtype=np.uint64)
+        ins[:, :, 0] = r_.integers(0, 2, size=(cnt, d.main.n_in), dtype=np.uint64)
+        c = Circuit(d, fuse=True)
+        bt = Batch(c, cnt)
+        bt.set_inputs(ins)
+        bt.run()
+        r = R1cs(c)
+        k, _ = r.qap_info()
+        n = 1 << k
+        if n > bls_np.shape[0]:
+            more, _ = BM.multiples(rng.randrange(BM.R), rng.randrange(BM.R), n)
+            bls_np = np.frombuffer(b"".join(x.to_bytes(48, "little") + y.to_bytes(48, "little") for x, y in more),
+                                   dtype=np.uint64).reshape(-1, 2, 6)
+            del more
+        g = Bls12381G1Bases(bls_np[:n])
+        stream = torch.cuda.ExternalStream(bt.stream())
+        h = torch.empty((cnt, n, 4), dtype=torch.int64, device="cuda")
+        qs = torch.empty((2 * cnt, n, 4), dtype=torch.int64, device="cuda")
+        out = torch.zeros((cnt, 2, 6), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(g.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        for rep in range(2):   # the first round is the warm-up
+            ev[0].record(stream)
+            r.quotient_batch(bt, 0, cnt, h.data_ptr(), qs.data_ptr())
+            ev[1].record(stream)
+            g.msm(h.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr(), bt.stream())
+            ev[2].record(stream)
+            bt.sync()
+        q_ms, m_ms = ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])
+        print(json.dumps({"what": "pipeline_bls12381", "circuit": "sha256_512", "log2_n": k, "witnesses": cnt,
+                          "quotient_ms_per_witness": round(q_ms / cnt, 3), "h_msm_ms_per_witness": round(m_ms / cnt, 3),
+                          "total_ms_per_witness": round((q_ms + m_ms) / cnt, 3)}), flush=True)
     print(json.dumps({"card_after": card()}), flush=True)
 
 
