@@ -9,9 +9,9 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcircom_b200.so")
 CLI = os.path.join(HERE, "circom_cuda_witness")
 PROVER = os.path.join(HERE, "circom_cuda_prover")
-SOURCES = ["capi.cu", "tape_calls.cu", "msm_g2.cu", "msm_bls12381.cu", "groth16.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
+SOURCES = ["capi.cu", "tape_calls.cu", "msm_g2.cu", "msm_bls12381.cu", "msm_bls12381_g2.cu", "groth16.cu", "flatten.cpp", "formats.cpp", "hostpack.cpp", "r1cs_compile.cpp"]
 CLI_SOURCES = ["cli.cpp", "prover_cli.cpp"]
-HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "msm_g2.cuh", "msm_g2.h", "msm_bls12381.cuh", "msm_bls12381.h", "groth16.cuh", "groth16.h", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
+HEADERS = ["kernels.cuh", "fr_device.cuh", "ntt.cuh", "msm.cuh", "msm_g2.cuh", "msm_g2.h", "msm_bls12381.cuh", "msm_bls12381.h", "msm_bls12381_g2.cuh", "msm_bls12381_g2.h", "groth16.cuh", "groth16.h", "tape.h", "tape_calls.h", "u256.h", "hostpack.h", "r1cs_small.h", os.path.join("..", "..", "include", "circom_b200.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-ldl"]
 

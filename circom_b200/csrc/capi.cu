@@ -32,6 +32,7 @@
 #include "msm.cuh"
 #include "msm_g2.h"
 #include "msm_bls12381.h"
+#include "msm_bls12381_g2.h"
 #include "groth16.h"
 #include "tape_calls.h"
 #include "tape.h"
@@ -119,6 +120,7 @@ int ensure_device(int device) {
         CU(tape_calls_set_params(h, sizeof(h)));
         CU(msm_g2_set_params(h, sizeof(h)));
         CU(msm_bls12381_set_params());
+        CU(msm_bls12381_g2_set_params());
         CU(groth16_set_params(h, sizeof(h)));
         g_dev_ready[device] = true;
     }
@@ -2172,6 +2174,89 @@ int cw_bls12381_g1_msm_batch(cw_bls12381_g1_bases *b, const uint64_t *scalars_de
         }
         msm_bls12381_launch_reduce(buckets, p.B, n_win, S + p.segs, S + p.wins, p.W, p.c, cn,
                                    (uint4 *)(out_dev + 12 * (size_t)i0), st);
+        CU(cudaGetLastError());
+    }
+    return CW_OK;
+}
+
+// ---- multi-scalar multiplication on G2 of BLS12-381 (msm_bls12381_g2.cuh, kernels in msm_bls12381_g2.cu) ------------
+struct cw_bls12381_g2_bases {
+    int device = 0;
+    uint64_t n = 0;
+    DevPtr<u32> pts;   // [n][48] u32: Montgomery x.c0, x.c1, y.c0, y.c1 (12 limbs each); all zeros = infinity
+};
+
+int cw_bls12381_g2_bases_create(const uint64_t *points, uint64_t n, int device, cw_bls12381_g2_bases **out) {
+    if (!out || (!points && n)) return fail(CW_EINVAL, "null argument");
+    *out = nullptr;
+    if (n == 0 || n > MSM_MAX_N) return fail(CW_EINVAL, "the number of points must lie in [1, 2^26]");
+    std::vector<u32> mont(48 * n);
+    for (uint64_t i = 0; i < n; ++i) {
+        int coef = 0;
+        const int bad = bls12381_g2_point_mont(points + 24 * i, &mont[48 * i], &coef);
+        if (bad == 1)
+            return fail(CW_EINVAL, "point " + std::to_string(i) + ": coefficient " + std::to_string(coef) +
+                                       " (x.c0, x.c1, y.c0, y.c1) is not below q");
+        if (bad) return fail(CW_EINVAL, "point " + std::to_string(i) + " is not on the twist y^2 = x^3 + 4 (1 + u)");
+    }
+    int rc = ensure_device(device);
+    if (rc) return rc;
+    auto b = std::make_unique<cw_bls12381_g2_bases>();
+    b->device = device;
+    b->n = n;
+    if ((rc = upload(b->pts, mont.data(), mont.size() * 4))) return rc;
+    *out = b.release();
+    return CW_OK;
+}
+
+void cw_bls12381_g2_bases_destroy(cw_bls12381_g2_bases *b) {
+    if (!b) return;
+    cudaSetDevice(b->device);
+    delete b;
+}
+
+int cw_bls12381_g2_msm_scratch_bytes(const cw_bls12381_g2_bases *b, uint32_t count, uint64_t *bytes) {
+    if (!b || !bytes || count == 0) return fail(CW_EINVAL, "bad argument");
+    int rc = ensure_device(b->device);
+    if (rc) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_BLS_G2_POINT_BYTES))) return rc;
+    *bytes = p.total;
+    return CW_OK;
+}
+
+int cw_bls12381_g2_msm_batch(cw_bls12381_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                             uint64_t *out_dev, void *scratch_dev, void *stream) {
+    if (!b) return fail(CW_EINVAL, "bad argument");
+    int rc = msm_check_args(b->n, scalars_dev, stride_elems, count, out_dev, scratch_dev);
+    if (rc) return rc;
+    if ((rc = ensure_device(b->device))) return rc;
+    if ((rc = msm_check_pointers(b->device, scalars_dev, out_dev, scratch_dev))) return rc;
+    MsmPlan p;
+    if ((rc = msm_plan_for(b->n, count, p, MSM_BLS_G2_POINT_BYTES))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    char *S = (char *)scratch_dev;
+    const u32 n = (u32)b->n;
+    for (u32 i0 = 0; i0 < count; i0 += p.chunk) {
+        const u32 cn = std::min(p.chunk, count - i0), n_win = cn * p.W;
+        const uint64_t N = (uint64_t)n_win * n;
+        if ((rc = msm_sorted_digits(p, S, scalars_dev, stride_elems, n, i0, cn, st))) return rc;
+        void *buckets = S + p.buckets;
+        CU(cudaMemsetAsync(buckets, 0, (size_t)n_win * p.B * MSM_BLS_G2_POINT_BYTES, st));
+        // level 0 over the sorted affine items, then levels over the partial sums until one thread covered a level
+        uint64_t threads = (N + MSM_RUN - 1) / MSM_RUN, items = N;
+        int lv = 0;
+        msm_bls12381_g2_launch_runs(true, (const u32 *)(S + p.keys[1]), (const u32 *)(S + p.vals[1]), b->pts.get(), nullptr, N,
+                                    p.c, buckets, (u32 *)(S + p.lv_keys[0]), S + p.lv_pts[0], st);
+        while (threads > 1) {
+            items = msm_level_out(items);
+            threads = (items + MSM_RUN - 1) / MSM_RUN;
+            msm_bls12381_g2_launch_runs(false, (const u32 *)(S + p.lv_keys[lv]), nullptr, nullptr, S + p.lv_pts[lv], items, p.c,
+                                        buckets, (u32 *)(S + p.lv_keys[lv ^ 1]), S + p.lv_pts[lv ^ 1], st);
+            lv ^= 1;
+        }
+        msm_bls12381_g2_launch_reduce(buckets, p.B, n_win, S + p.segs, S + p.wins, p.W, p.c, cn,
+                                      (uint4 *)(out_dev + 24 * (size_t)i0), st);
         CU(cudaGetLastError());
     }
     return CW_OK;

@@ -364,7 +364,7 @@ struct MsmBlsXyzzItems {
 
 }  // namespace cw
 
-#if defined(__CUDACC__)
+#if defined(__CUDACC__) && !defined(CW_MSM_NO_BLS_G1_KERNELS)   // (msm_bls12381_g2.cu uses the field functions only)
 // ---- kernels (sm_90a) -------------------------------------------------------------------------------------------------
 // The digits and the sort are msm.cuh's (they do not depend on the group).  The bucket type is 1.5 times the BN254 G1
 // one over a product with 2.25 times the limb products, so the kernels run MSM_BLS_THREADS threads per CTA, which lets

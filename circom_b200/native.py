@@ -103,6 +103,10 @@ def _load() -> ctypes.CDLL:
         "cw_bls12381_g1_bases_destroy": (None, [P]),
         "cw_bls12381_g1_msm_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
         "cw_bls12381_g1_msm_batch": (c_int, [P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
+        "cw_bls12381_g2_bases_create": (c_int, [c_void_p, c_uint64, c_int, POINTER(P)]),
+        "cw_bls12381_g2_bases_destroy": (None, [P]),
+        "cw_bls12381_g2_msm_scratch_bytes": (c_int, [P, c_uint32, POINTER(c_uint64)]),
+        "cw_bls12381_g2_msm_batch": (c_int, [P, c_void_p, c_uint64, c_uint32, c_void_p, c_void_p, c_void_p]),
         "cw_groth16_key_create": (c_int, [c_void_p, c_size_t, P, c_int, POINTER(P)]),
         "cw_groth16_key_destroy": (None, [P]),
         "cw_groth16_key_info": (c_int, [P, POINTER(c_uint64)]),

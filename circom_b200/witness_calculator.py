@@ -680,6 +680,67 @@ class Bls12381G1Bases:
         return self.decode(out.cpu().numpy().view(np.uint64))
 
 
+class Bls12381G2Bases:
+    """BLS12-381 G2 points (on the twist y^2 = x^3 + 4 (1 + u) over Fq2) on the device for multi-scalar multiplications
+    (cw_bls12381_g2_bases_*, include/circom_b200.h).  points: numpy uint64 [n][2][2][6] canonical affine (x.c0, x.c1, y.c0,
+    y.c1, 6 limbs each), or a list of ((x0, x1), (y0, y1)) ints; all zeros or None is the point at infinity.  Points are
+    checked to lie on the twist, not to lie in the order-r subgroup.  Scalars are [count][n][4] uint64, as for G2Bases."""
+
+    def __init__(self, points, device: int = 0):
+        if isinstance(points, np.ndarray):
+            arr = np.ascontiguousarray(points, dtype=np.uint64).reshape(-1, 2, 2, 6)
+        else:
+            arr = np.zeros((len(points), 2, 2, 6), dtype=np.uint64)
+            for i, p in enumerate(points):
+                for j, e in enumerate(((0, 0), (0, 0)) if p is None else p):
+                    for k, v in enumerate(e):
+                        arr[i, j, k] = [(v >> (64 * m)) & 0xFFFFFFFFFFFFFFFF for m in range(6)]
+        self.n = arr.shape[0]
+        self.device = device
+        self._h = ctypes.c_void_p()
+        check(lib.cw_bls12381_g2_bases_create(arr.ctypes.data, self.n, device, ctypes.byref(self._h)))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            lib.cw_bls12381_g2_bases_destroy(h)
+
+    def scratch_bytes(self, count: int) -> int:
+        b = ctypes.c_uint64()
+        check(lib.cw_bls12381_g2_msm_scratch_bytes(self._h, count, ctypes.byref(b)))
+        return b.value
+
+    def msm(self, scalars_ptr: int, stride: int, count: int, out_ptr: int, scratch_ptr: int, stream=None) -> None:
+        """out[c] = sum_i s_{c,i} Q_i into device [count][2][2][6] uint64; scalars: device [count][stride][4] uint64.
+        Asynchronous on `stream` (a Batch.stream() value; None = the legacy default stream)."""
+        check(lib.cw_bls12381_g2_msm_batch(self._h, ctypes.c_void_p(scalars_ptr), stride, count, ctypes.c_void_p(out_ptr),
+                                           ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream or None)))
+
+    @staticmethod
+    def decode(out: np.ndarray) -> List[Optional[tuple]]:
+        """[count][2][2][6] uint64 results -> [((x0, x1), (y0, y1)) or None per vector]"""
+        a = np.ascontiguousarray(out, dtype=np.uint64).reshape(-1, 6)
+        v = [sum(int(r[k]) << (64 * k) for k in range(6)) for r in a]
+        return [None if not any(v[i:i + 4]) else ((v[i], v[i + 1]), (v[i + 2], v[i + 3])) for i in range(0, len(v), 4)]
+
+    def msm_host(self, scalars) -> List[Optional[tuple]]:
+        """the MSMs of host scalars ([count][n] ints, or numpy uint64 [count][n][4]): [((x0, x1), (y0, y1)) or None]"""
+        import torch
+        if isinstance(scalars, np.ndarray):
+            arr = np.ascontiguousarray(scalars, dtype=np.uint64).reshape(-1, self.n, 4)
+        else:
+            arr = np.array([[[(s >> (64 * k)) & 0xFFFFFFFFFFFFFFFF for k in range(4)] for s in row] for row in scalars],
+                           dtype=np.uint64).reshape(-1, self.n, 4)
+        count = arr.shape[0]
+        dev = torch.device("cuda", self.device)
+        s = torch.from_numpy(arr.view(np.int64)).to(dev)
+        out = torch.zeros((count, 2, 2, 6), dtype=torch.int64, device=dev)
+        scratch = torch.empty(self.scratch_bytes(count), dtype=torch.uint8, device=dev)
+        self.msm(s.data_ptr(), self.n, count, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize(dev)
+        return self.decode(out.cpu().numpy().view(np.uint64))
+
+
 def _proof_from_limbs(v: Sequence[int]):
     """one proof's 8 canonical coordinates -> (A, B, C): A, C = (x, y), B = ((x0, x1), (y0, y1)); None = infinity"""
     A = None if not any(v[0:2]) else (v[0], v[1])

@@ -9,8 +9,8 @@
  * elements crossing the ABI are CANONICAL integers in [0,q) as 4 little-endian
  * uint64 limbs (the same 32 bytes the reference writes to .wtns,
  * c_elements/common/main.cpp:328-332).  Montgomery form is internal.  The one
- * exception is the base field of BLS12-381 G1 (381 bits): its coordinates are
- * 6 little-endian uint64 limbs (cw_bls12381_g1_*).
+ * exception is the base field of BLS12-381 (381 bits): its coordinates are
+ * 6 little-endian uint64 limbs (cw_bls12381_g1_*, cw_bls12381_g2_*).
  *
  * Error convention: functions return CW_OK (0) or a negative CW_E* code;
  * cw_last_error() gives a thread-local message.  The reference instead
@@ -382,6 +382,34 @@ int cw_bls12381_g1_msm_scratch_bytes(const cw_bls12381_g1_bases *b, uint32_t cou
 /* out_dev[c] = sum_{i<n} s_{c,i} P_i for c < count, affine canonical ([count][2][6] u64, (0, 0) = infinity).
  * Scalars ([count][stride][4] u64), strides, alignment, devices and streams as for cw_g1_msm_batch. */
 int cw_bls12381_g1_msm_batch(cw_bls12381_g1_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
+                             uint64_t *out_dev, void *scratch_dev, void *stream);
+
+/* ---- multi-scalar multiplication on G2 of BLS12-381 ------------------------------------------------------------------
+ * The B2 MSM of a BLS12-381 prover, sum_i w_i Q_i over the proving key's G2 points, after cw_batch_expand_witness of a
+ * circuit over the bls12381 prime.
+ *   G2 of BLS12-381 is taken on the twist E': y^2 = x^3 + 4 (1 + u) over Fq2 = Fq[u] / (u^2 + 1), q the 381-bit base
+ *   field of G1 above.  The subgroup of order r is G2; #E'(Fq2) = h2 r with the odd 507-bit cofactor
+ *   h2 = 0x5d543a95414e7f1091d50792876a202cd91de4547085abaa68a205b2e5a7ddfa628f1cb4d9e82ef21537e293a6691ae1616ec6e786f0c70cf1c38e31c7238e5.
+ *   A point at the ABI is affine, [2][2][6] u64 canonical: x.c0, x.c1, y.c0, y.c1, each 6 little-endian limbs, 192 bytes
+ *   per point; c0 comes first, as in the BN254 G2 layout.  The point at infinity is all zeros, which is not on E'
+ *   (b' != 0).
+ *   Points are checked to lie on E', not to lie in the order-r subgroup (that costs a scalar multiplication per point).
+ *   The result is the exact sum sum_i s_i Q_i in E'(Fq2) for any points on E', with s_i taken as a 256-bit integer;
+ *   "s and s mod r give the same point" holds for points of the subgroup only.
+ * The calls mirror the BLS12-381 G1 and the BN254 G2 ones above. */
+typedef struct cw_bls12381_g2_bases cw_bls12381_g2_bases;
+/* n points (host memory, [n][2][2][6] u64 canonical affine) uploaded to `device` once.  Every point must be all zeros or
+ * have its four coefficients below q and lie on E'; otherwise CW_EINVAL, and cw_last_error names the first bad index (and,
+ * for a coefficient not below q, which coefficient).  These checks run on the host before any device is touched.
+ * 1 <= n <= 2^26.  No device: CW_ENODEV. */
+int cw_bls12381_g2_bases_create(const uint64_t *points, uint64_t n, int device, cw_bls12381_g2_bases **out);
+void cw_bls12381_g2_bases_destroy(cw_bls12381_g2_bases *b);
+/* device scratch that cw_bls12381_g2_msm_batch needs for `count` scalar vectors (chunks of about 2 GB, as for BN254; at
+ * n = 2^21 one instance's plan is about 2.0 GB, so a chunk holds one instance) */
+int cw_bls12381_g2_msm_scratch_bytes(const cw_bls12381_g2_bases *b, uint32_t count, uint64_t *bytes);
+/* out_dev[c] = sum_{i<n} s_{c,i} Q_i for c < count, affine canonical ([count][2][2][6] u64, all zeros = infinity).
+ * Scalars ([count][stride][4] u64), strides, alignment, devices and streams as for cw_g1_msm_batch. */
+int cw_bls12381_g2_msm_batch(cw_bls12381_g2_bases *b, const uint64_t *scalars_dev, uint64_t stride_elems, uint32_t count,
                              uint64_t *out_dev, void *scratch_dev, void *stream);
 
 /* ---- Groth16 proofs on BN254 -----------------------------------------------------------------------------------------

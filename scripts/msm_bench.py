@@ -6,6 +6,8 @@ Prints, per shape, ms per MSM (CUDA events after a warm-up of that shape) and a 
 chosen plan performs whatever the scalars (counted below from n, c, the scalars' nonzero digits and the formula costs of
 csrc/msm.cuh, csrc/msm_g2.cuh: an Fq2 product is 3 products, a square 2) over the product rate cw_fr_mul_bench measures in the same call.  That probe is built for bn128's scalar field; the MSM multiplies
 in the base field q, which has the same 254-bit size and the same product code, so the bn128 rate stands in for it.
+With --group bls12381 / bls12381-g2, the BLS12-381 G1 / G2 MSMs beside the BN254 ones (and, for G2, the BLS12-381 G1
+one) of the same shape and scalars.
 Scalar kinds: uniform random 256-bit values, and expanded Sha256compression witness rows tiled to n (mostly bits).
 The card's name, power limit and SM clock are read in the same call.  One JSON object per line.
 """
@@ -74,15 +76,19 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--sweep", default="20:14-19,21:15-19", help="log2 n:c range pairs timed at count 8, uniform scalars")
     ap.add_argument("--pipeline", type=int, default=64, help="headline witnesses for quotient + H MSM (0: skip)")
-    ap.add_argument("--group", choices=("g1", "g2", "bls12381"), default="g1",
+    ap.add_argument("--group", choices=("g1", "g2", "bls12381", "bls12381-g2"), default="g1",
                     help="g2: time cw_g2_msm_batch, and the pipeline leg is B1 + B2 over expanded headline witness rows; "
                          "bls12381: time cw_bls12381_g1_msm_batch beside cw_g1_msm_batch of the same shape, and the "
-                         "pipeline leg is quotient + H MSM of BLS12-381 Sha256(512) (config C4)")
+                         "pipeline leg is quotient + H MSM of BLS12-381 Sha256(512) (config C4); bls12381-g2: time "
+                         "cw_bls12381_g2_msm_batch beside cw_g2_msm_batch and cw_bls12381_g1_msm_batch of the same shape, "
+                         "and the pipeline leg is witness expansion + B2 MSM of config C4")
     args = ap.parse_args()
     if args.group == "g2":
         return main_g2(args)
     if args.group == "bls12381":
         return main_bls(args)
+    if args.group == "bls12381-g2":
+        return main_bls_g2(args)
     import torch
     from circom_b200 import native
     from circom_b200.circuit import CircuitDesc
@@ -475,6 +481,158 @@ def main_bls(args):
         print(json.dumps({"what": "pipeline_bls12381", "circuit": "sha256_512", "log2_n": k, "witnesses": cnt,
                           "quotient_ms_per_witness": round(q_ms / cnt, 3), "h_msm_ms_per_witness": round(m_ms / cnt, 3),
                           "total_ms_per_witness": round((q_ms + m_ms) / cnt, 3)}), flush=True)
+    print(json.dumps({"card_after": card()}), flush=True)
+
+
+MADD_G1, ADD_G1 = 10, 14   # 381-bit products of the G1 formulas (msm_bls12381.cuh)
+MADD_F2, ADD_F2 = 28, 40   # the same over Fq2 (msm_bls12381_g2.cuh, msm_g2.cuh): an Fq2 product is 3 products, a square 2
+
+
+def main_bls_g2(args):
+    """BLS12-381 G2 against BN254 G2 and BLS12-381 G1 at the same shapes and scalars, in the same call.  Expected ratios
+    from the integer work alone: BN254 G2 runs the same Fq2 formulas on 8-limb products, (12/8)^2 = 2.25 times less work
+    per product; BLS12-381 G1 runs the same 12-limb product, 28 / 10 times fewer of them per mixed addition.  They are
+    printed next to the measured ratios as expectations, not as bounds.  The scratch of one instance and the instances per
+    chunk (about 2 GB of scratch) are printed per size."""
+    import torch
+    from circom_b200.circuit import CircuitDesc
+    from circom_b200 import circuits as C
+    from circom_b200.witness_calculator import Circuit, Batch, Bls12381G1Bases, Bls12381G2Bases, G2Bases, limbs_to_ints
+    from oracle import g2_model as M2
+    from tests import bls12381_g2_model as BM2
+    from tests import bls12381_model as BM
+
+    print(json.dumps({"card": card(), "group": "bls12381-g2"}), flush=True)
+    logs = [int(x) for x in args.logs.split(",")]
+    counts = [int(x) for x in args.counts.split(",")]
+    n_max = 1 << max(logs + [21])
+    rng = random.Random(1)
+    to_np = lambda pts, nb, shape: np.frombuffer(b"".join(c.to_bytes(nb, "little") for p in pts for e in p for c in e),
+                                                 dtype=np.uint64).reshape(shape)
+    pts, _ = BM2.multiples_g2(rng.randrange(BM.R), rng.randrange(BM.R), n_max)
+    g2_np = to_np(pts, 48, (-1, 2, 2, 6))
+    pts, _ = M2.multiples(rng.randrange(M2.R), rng.randrange(M2.R), n_max)
+    bn2_np = to_np(pts, 32, (-1, 2, 2, 4))
+    pts, _ = BM.multiples(rng.randrange(BM.R), rng.randrange(BM.R), n_max)
+    g1_np = np.frombuffer(b"".join(x.to_bytes(48, "little") + y.to_bytes(48, "little") for x, y in pts),
+                          dtype=np.uint64).reshape(-1, 2, 6)
+    del pts
+
+    # bit-heavy rows: expanded BLS12-381 Sha256compression witnesses
+    d = CircuitDesc("bls12381")
+    d.set_main(C.sha256_compression(d))
+    sc = Circuit(d, fuse=True)
+    sb = Batch(sc, max(counts))
+    ins = np.zeros((max(counts), sc.n_inputs, 4), dtype=np.uint64)
+    ins[:, :, 0] = np.random.default_rng(0).integers(0, 2, size=(max(counts), sc.n_inputs), dtype=np.uint64)
+    sb.set_inputs(ins)
+    sb.run()
+    wrows = sb.witness()
+    del sb
+
+    def time_msm(b, s, n, cnt, shape):
+        out = torch.zeros((cnt,) + shape, dtype=torch.int64, device="cuda")
+        scratch = torch.empty(b.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(args.reps):
+            b.msm(s.data_ptr(), n, cnt, out.data_ptr(), scratch.data_ptr())
+        e1.record()
+        torch.cuda.synchronize()
+        del scratch
+        return e0.elapsed_time(e1) / args.reps
+
+    for k in logs:
+        n = 1 << k
+        gb, bn2, g1 = Bls12381G2Bases(g2_np[:n]), G2Bases(bn2_np[:n]), Bls12381G1Bases(g1_np[:n])
+        c = window_bits(n)
+        one = gb.scratch_bytes(1)
+        print(json.dumps({"what": "bls12381_g2_plan", "log2_n": k, "c": c, "scratch_bytes_one_instance": one,
+                          "instances_per_chunk": max(1, (2 << 30) // one)}), flush=True)
+        for kind in ("uniform", "bits"):
+            for cnt in counts:
+                if kind == "uniform":
+                    s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+                    live = cnt * n * windows(c)
+                else:
+                    reps = -(-n // wrows.shape[1])
+                    host = np.concatenate([np.tile(wrows[i % wrows.shape[0]], (reps, 1))[:n][None] for i in range(cnt)])
+                    s = torch.from_numpy(host.view(np.int64)).cuda()
+                    live = 0
+                    for i in range(cnt):
+                        row = limbs_to_ints(wrows[i % wrows.shape[0]])
+                        per = sum(nonzero_digits(v, c) for v in row)
+                        full, part = divmod(n, len(row))
+                        live += full * per + sum(nonzero_digits(v, c) for v in row[:part])
+                ms = time_msm(gb, s, n, cnt, (2, 2, 6))
+                ms_bn2 = time_msm(bn2, s, n, cnt, (2, 2, 4))
+                ms_g1 = time_msm(g1, s, n, cnt, (2, 6))
+                print(json.dumps({"what": "bls12381_g2_msm", "scalars": kind, "log2_n": k, "c": c, "count": cnt,
+                                  "ms_call": round(ms, 3), "ms_per_msm": round(ms / cnt, 3),
+                                  "p381_products_per_msm": products(n, c, live // cnt, MADD_F2, DBL_G2),
+                                  "bn254_g2_ms_per_msm": round(ms_bn2 / cnt, 3),
+                                  "bls12381_g1_ms_per_msm": round(ms_g1 / cnt, 3),
+                                  "over_bn254_g2": round(ms / ms_bn2, 2), "limb_work_ratio_expected": 2.25,
+                                  "over_bls12381_g1": round(ms / ms_g1, 2),
+                                  "product_ratio_expected": round(MADD_F2 / MADD_G1, 2)}), flush=True)
+                del s
+                torch.cuda.empty_cache()
+        del gb, bn2, g1
+        torch.cuda.empty_cache()
+
+    for part in filter(None, args.sweep.split(",")):
+        k, rng_c = part.split(":")
+        lo, hi = (int(x) for x in rng_c.split("-"))
+        n, cnt = 1 << int(k), 8
+        b = Bls12381G2Bases(g2_np[:n])
+        s = torch.randint(-2**63, 2**63 - 1, (cnt, n, 4), dtype=torch.int64, device="cuda")
+        for c in range(lo, hi + 1):
+            os.environ["CW_MSM_WINDOW"] = str(c)
+            ms = time_msm(b, s, n, cnt, (2, 2, 6))
+            print(json.dumps({"what": "window_sweep_bls12381_g2", "log2_n": int(k), "c": c, "rule_c": window_bits(n),
+                              "count": cnt, "ms_per_msm": round(ms / cnt, 3)}), flush=True)
+        os.environ.pop("CW_MSM_WINDOW", None)
+        del b, s
+        torch.cuda.empty_cache()
+
+    # the pipeline leg of config C4 (Sha256 of 512 bits over BLS12-381): witness expansion, then the B2 MSM on the batch
+    # stream
+    if args.pipeline:
+        cnt = args.pipeline
+        d = CircuitDesc("bls12381")
+        d.set_main(C.sha256(d, 512))
+        r_ = np.random.default_rng(0)
+        ins = np.zeros((cnt, d.main.n_in, 4), dtype=np.uint64)
+        ins[:, :, 0] = r_.integers(0, 2, size=(cnt, d.main.n_in), dtype=np.uint64)
+        c = Circuit(d, fuse=True)
+        bt = Batch(c, cnt)
+        bt.set_inputs(ins)
+        bt.run()
+        nw = c.n_witness
+        if nw > g2_np.shape[0]:
+            more, _ = BM2.multiples_g2(rng.randrange(BM.R), rng.randrange(BM.R), nw)
+            g2_np = to_np(more, 48, (-1, 2, 2, 6))
+            del more
+        g = Bls12381G2Bases(g2_np[:nw])
+        stream = torch.cuda.ExternalStream(bt.stream())
+        rows = torch.empty((cnt, nw, 4), dtype=torch.int64, device="cuda")
+        out = torch.zeros((cnt, 2, 2, 6), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(g.scratch_bytes(cnt), dtype=torch.uint8, device="cuda")
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        for rep in range(2):   # the first round is the warm-up
+            ev[0].record(stream)
+            bt.expand_witness(0, cnt, rows.data_ptr())
+            ev[1].record(stream)
+            g.msm(rows.data_ptr(), nw, cnt, out.data_ptr(), scratch.data_ptr(), bt.stream())
+            ev[2].record(stream)
+            bt.sync()
+        e_ms, m_ms = ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])
+        print(json.dumps({"what": "pipeline_bls12381_b2", "circuit": "sha256_512", "n_witness": nw, "c": window_bits(nw),
+                          "witnesses": cnt, "expand_ms_per_witness": round(e_ms / cnt, 3),
+                          "b2_msm_ms_per_witness": round(m_ms / cnt, 3),
+                          "total_ms_per_witness": round((e_ms + m_ms) / cnt, 3)}), flush=True)
     print(json.dumps({"card_after": card()}), flush=True)
 
 
